@@ -319,7 +319,8 @@ typedef struct PbrtStats {
     uint32_t trace_launches;
     uint32_t kernel_launches;
     /* ABI v4 */
-    uint64_t shade_slots;     /* queue slots the shade kernel processed (path vertices + pending next-event estimates) */
+    uint64_t shade_slots;     /* queue slots the shade kernel processed (surface hits only: a slot whose path ray missed, or whose path
+                                 already ended, is finished by the sort kernel before it, pending next-event estimate included) */
     uint64_t shaded_vertices; /* of those, surface hits it shaded (PathIntegrator::li loop bodies that reached a BSDF or a null surface) */
 } PbrtStats;
 

@@ -426,10 +426,12 @@ __global__ void __launch_bounds__(256) k_rayprep(const float4* __restrict__ rays
     }
 }
 
-// k_sort: bucket the slots of the shade queue by what k_shade has to do with them -- class 0: no surface to
-// shade (the path ray missed, or the path already ended and only its pending NEE has to be resolved);
-// class c >= 1: hit on a material of shading class c (same lobe-kind sequence => same code path, warp ballot /
-// match + prefix sum).  Also raises the spatial light distribution's voxel requests for the hits
+// k_sort: everything the traced rays leave to do before the next surface is shaded, then the bucketing of those surface hits for
+// k_shade.  First the previous vertex's estimate_direct is finished with the shadow / MIS results (integrator.rs:461-567), then a path
+// ray that escaped adds the environment emission (path.rs:267-275): the reference adds both before the Le of the next vertex, so they
+// come first here too.  A slot without a surface hit is then finished -- L is final, its flags are 0 -- and joins no queue.  A hit goes
+// to class c >= 1, the shading class of its material (same lobe-kind sequence => same code path; warp match + prefix sum); null-
+// material hits go to class 1.  Also raises the spatial light distribution's voxel requests for the hits
 // (the lookup of path.rs:118; extra requests are harmless, the distribution of a voxel is deterministic).
 // The counters the NEXT kernels append to are reset here rather than by memsets between the launches (five per iteration before):
 // k_sort clears the survivor count and the ray count k_shade is about to fill, k_shade clears what the next iteration's k_trace /
@@ -445,11 +447,47 @@ __global__ void __launch_bounds__(256) k_sort(DScene sc, DPaths ps, DLightGrid g
         uint32_t cls = 0xffffffffu, slot = 0;
         if (qi < count) {
             slot = queue[qi];
-            cls = 0;
-            if (__float_as_uint(ps.L[slot].w) & PF_HAS_RAY) {
+            const float4 Lf = ps.L[slot];
+            const uint32_t flags = __float_as_uint(Lf.w);
+            Sp L = mksp(Lf.x, Lf.y, Lf.z);
+            if (flags & (PF_HAS_SHADOW | PF_HAS_MIS)) {  // the next-event estimate of the previous vertex
+                Sp ld = sp1(0.0f);
+                const float4 a = ps.ld_light[slot];
+                if ((flags & PF_HAS_SHADOW) && ps.occl[slot] == 0u) ld = ld + mksp(a.x, a.y, a.z);
+                if (flags & PF_HAS_MIS) {
+                    const float4 mh = ps.mis_hit[slot];
+                    int mprim = __float_as_int(mh.x);
+                    if (mprim >= 0) {
+                        const float4 md = ps.mis_d[slot], mf = ps.mis_f[slot];
+                        int light_num = (int)__float_as_uint(md.w);
+                        V3 lp, ln;
+                        int hit_light;
+                        tri_point_normal(sc, (uint32_t)mprim, mh.y, mh.z, mh.w, lp, ln, hit_light);
+                        if (hit_light == light_num) {
+                            Sp le = light_L(sc.lights[light_num], ln, -mk3(md.x, md.y, md.z));
+                            if (!is_black(le)) ld = ld + mksp(mf.x, mf.y, mf.z) * le * sp1(1.0f) * a.w / mf.w;
+                        }
+                    } else if (sc.n_inf) {  // the MIS ray left the scene: li = light.le(ray) (integrator.rs:560-562)
+                        const float4 md = ps.mis_d[slot], mf = ps.mis_f[slot];
+                        Sp le = light_le(sc, sc.lights[__float_as_uint(md.w)], mk3(md.x, md.y, md.z));
+                        if (!is_black(le)) ld = ld + mksp(mf.x, mf.y, mf.z) * le * sp1(1.0f) * a.w / mf.w;
+                    }
+                }
+                const float4 nb = ps.nee_beta[slot];
+                L = L + mksp(nb.x, nb.y, nb.z) * spdiv0(ld, nb.w);  // ld is black for every occluded light sample
+            }
+            if (flags & PF_HAS_RAY) {
                 float4 h = ps.hit[slot];
                 int prim = __float_as_int(h.x);
-                if (prim >= 0) {
+                if (prim < 0) {
+                    // the path ray escaped: environment emission (path.rs:267-275)
+                    if (sc.n_inf && ((flags >> PF_BOUNCES_SHIFT) == 0 || (flags & PF_SPECULAR_BOUNCE))) {
+                        const float4 b4 = ps.beta[slot], rd4 = ps.ray_d[slot];
+                        const Sp beta = mksp(b4.x, b4.y, b4.z);
+                        const V3 rd = mk3(rd4.x, rd4.y, rd4.z);
+                        for (uint32_t k = 0; k < sc.n_inf; ++k) L = L + beta * light_le(sc, sc.lights[sc.inf[k]], rd);
+                    }
+                } else {
                     float4 c = __ldg(sc.tri_verts + 3 * (size_t)prim + 2);
                     uint32_t mat = __float_as_uint(c.y);
                     const uint32_t inst = sc.n_instances ? ps.hit_inst[slot] : 0xffffffffu;
@@ -478,6 +516,8 @@ __global__ void __launch_bounds__(256) k_sort(DScene sc, DPaths ps, DLightGrid g
                     }
                 }
             }
+            if (cls == 0xffffffffu) ps.L[slot] = make_float4(L.r, L.g, L.b, __uint_as_float(0u));
+            else if (flags & (PF_HAS_SHADOW | PF_HAS_MIS)) ps.L[slot] = make_float4(L.r, L.g, L.b, __uint_as_float(flags & ~(PF_HAS_SHADOW | PF_HAS_MIS)));
         }
         // one atomic per distinct class in the warp
         unsigned peers = __match_any_sync(0xffffffffu, cls);
@@ -684,8 +724,8 @@ __global__ void __launch_bounds__(256) k_ray_scatter2(const uint32_t* __restrict
 }
 
 // -----------------------------------------------------------------------------------------------
-// k_shade: (1) finish the previous vertex's estimate_direct with the traced shadow / MIS results
-// (integrator.rs:461-567), (2) shade one path vertex: path.rs:95-279, integrator.rs:359-570.
+// k_shade: shade one path vertex, a surface hit k_sort filed under a shading class: path.rs:95-279, integrator.rs:359-570 (k_sort
+// has already finished the previous vertex's estimate_direct).
 // Material::compute_scattering_functions of a material with image textures at one hit (e.g. matte.rs:52-86): the bump map first
 // (Material::bump, material.rs:116-219, + set_shading_geometry, interaction.rs:345-370: `is` leaves with the new shading frame), then
 // the bound textures, then the lobe list of this hit.  Shared by k_texture and the direct / whitted kernels.
@@ -775,10 +815,12 @@ __global__ void __launch_bounds__(128) k_texture(DScene sc, DRender rp, DPaths p
 // instance-free scenes run, so that their code is the measured one.
 // SPEC = 1 + k: the instantiation for the shading class "a single lobe of kind k" -- untextured matte (Lambert / Oren-Nayar), metal,
 // substrate, mirror, smooth glass -- with the BSDF code folded to that one lobe (pb_bsdf.cuh): a fraction of the general kernel's
-// instructions.  The host launches one instantiation per class the scene has (class 0, "nothing to shade", rides with the first) and
+// instructions.  The host launches one instantiation per class the scene has and
 // the general one (SPEC = 0) over the multi-lobe / textured classes that are left; [cls_lo, cls_hi) is the launch's class range.
 #ifndef PB_SHADE_SPEC_BLOCKS
-#define PB_SHADE_SPEC_BLOCKS 4  // resident CTAs per SM the specialised instantiation is compiled for (register budget 65536 / (128 * n))
+// Resident CTAs per SM the specialised instantiation is compiled for (register budget 65536 / (128 * n)).  5 and 6 make ptxas spill
+// (104-200 B of stack) and were slower on the statue, Cornell and the conference scene on an H100 SXM (700 W).
+#define PB_SHADE_SPEC_BLOCKS 4
 #endif
 template <bool AREA_ONLY, bool HALTON, bool INST, int SPEC>
 __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_BLOCKS : 4)) k_shade(DScene sc, DRender rp, DPaths ps, DLightGrid grid, const uint32_t* __restrict__ nib,
@@ -828,8 +870,7 @@ __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_B
     const uint32_t warp_id = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     for (uint32_t tile = warp_id; tile < total_tiles; tile += warps_total) {
-        // every warp handles 32 slots of ONE class: warps never mix "nothing to shade" with surface shading, nor
-        // two lobe sets
+        // every warp handles 32 slots of ONE class: warps never mix two lobe sets
         uint32_t cls = 0;
         while (cls + 1 < PB_SHADE_CLASSES && tile >= s_tiles[cls + 1]) ++cls;
         const uint32_t qi = (tile - s_tiles[cls]) * 32u + lane;
@@ -841,230 +882,187 @@ __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_B
         if (qi < count) {
             slot = cls_queue[(size_t)cls * cls_stride + qi];
             n_slots++;
-            // all per-slot state is fetched up front, unconditionally, so that the loads overlap (the kernel is
-            // latency bound; records that turn out to be unused were written by an earlier bounce or are stale)
+            // all per-slot state is fetched up front so that the loads overlap (the kernel is latency bound)
             const float4 Lf = ps.L[slot];
             const float4 st_hit = ps.hit[slot], st_rd = ps.ray_d[slot], st_beta = ps.beta[slot];
             const uint2 st_sobol = ps.sobol[slot];
             const uint32_t st_dim = ps.dim[slot];
-            const float4 st_ld = ps.ld_light[slot], st_mh = ps.mis_hit[slot], st_md = ps.mis_d[slot], st_mf = ps.mis_f[slot], st_nb = ps.nee_beta[slot];
-            const uint32_t st_occl = ps.occl[slot];
             uint32_t flags = __float_as_uint(Lf.w);
             Sp L = mksp(Lf.x, Lf.y, Lf.z);
-            // ---- (1) next-event estimate of the previous vertex ------------------------------------
-            if (flags & (PF_HAS_SHADOW | PF_HAS_MIS)) {
-                Sp ld = sp1(0.0f);
-                const float4 a = st_ld;
-                if ((flags & PF_HAS_SHADOW) && st_occl == 0u) ld = ld + mksp(a.x, a.y, a.z);
-                if (flags & PF_HAS_MIS) {
-                    const float4 mh = st_mh;
-                    int mprim = __float_as_int(mh.x);
-                    if (mprim >= 0) {
-                        const float4 md = st_md, mf = st_mf;
-                        int light_num = (int)__float_as_uint(md.w);
-                        V3 lp, ln;
-                        int hit_light;
-                        tri_point_normal(sc, (uint32_t)mprim, mh.y, mh.z, mh.w, lp, ln, hit_light);
-                        if (hit_light == light_num) {
-                            Sp le = light_L(sc.lights[light_num], ln, -mk3(md.x, md.y, md.z));
-                            if (!is_black(le)) ld = ld + mksp(mf.x, mf.y, mf.z) * le * sp1(1.0f) * a.w / mf.w;
-                        }
-                    } else if (!AREA_ONLY && sc.n_inf) {  // the MIS ray left the scene: li = light.le(ray) (integrator.rs:560-562)
-                        const float4 md = st_md, mf = st_mf;
-                        Sp le = light_le(sc, sc.lights[__float_as_uint(md.w)], mk3(md.x, md.y, md.z));
-                        if (!is_black(le)) ld = ld + mksp(mf.x, mf.y, mf.z) * le * sp1(1.0f) * a.w / mf.w;
-                    }
-                }
-                const float4 nb = st_nb;
-                L = L + mksp(nb.x, nb.y, nb.z) * spdiv0(ld, nb.w);  // ld is black for every occluded light sample
-            }
             uint32_t out_flags = 0;  // terminated unless set below
-            // ---- (2) the vertex found by the path ray ------------------------------------------------
-            if (!AREA_ONLY && cls == 0u && sc.n_inf && (flags & PF_HAS_RAY) && __float_as_int(st_hit.x) < 0) {
-                // the path ray escaped: environment emission (path.rs:267-275)
-                if ((flags >> PF_BOUNCES_SHIFT) == 0 || (flags & PF_SPECULAR_BOUNCE)) {
-                    const Sp beta = mksp(st_beta.x, st_beta.y, st_beta.z);
-                    const V3 rd = mk3(st_rd.x, st_rd.y, st_rd.z);
-                    for (uint32_t k = 0; k < sc.n_inf; ++k) L = L + beta * light_le(sc, sc.lights[sc.inf[k]], rd);
-                }
+            uint32_t bounces = flags >> PF_BOUNCES_SHIFT;
+            bool specular_bounce = (flags & PF_SPECULAR_BOUNCE) != 0;
+            const float4 hit = st_hit;
+            int prim = __float_as_int(hit.x);  // k_sort files surface hits only: PF_HAS_RAY is set and prim >= 0
+            n_vertices++;
+            const float4 rd4 = st_rd, b4 = st_beta;
+            V3 rd = mk3(rd4.x, rd4.y, rd4.z);
+            Sp beta = mksp(b4.x, b4.y, b4.z);
+            float eta_scale = b4.w;
+            V3 wo = -rd;
+            V3 wo_nee = wo;  // isect.wo: what estimate_direct evaluates the BSDF with (differs for a transformed instance hit)
+            Isect is = INST ? hit_interaction(sc, rp.instancing, (uint32_t)prim, hit.y, hit.z, hit.w, ps.hit_inst[slot], rd, wo_nee)
+                                      : tri_interaction(sc, (uint32_t)prim, hit.y, hit.z, hit.w);
+            if (bounces == 0 || specular_bounce) {
+                // `l += beta * isect.le(&-ray.d)` (path.rs:97-100) also for a surface that emits nothing: le() is then black (interaction.rs:475-483),
+                // and beta * 0 is NaN when a degenerate BSDF value has made a component of beta infinite.  (The reference asserts on an infinite
+                // beta.y() right after the update, path.rs:158-171, so it aborts before it gets here; the oracle restates the arithmetic without
+                // the asserts, and this statement keeps the two restatements equal there too: the sample ends as NaN and k_resolve's has_nans()
+                // drops it -- tests/test_emu_kernels.py::test_randomised_materials_and_settings.)
+                const Sp le = is.area_light >= 0 ? light_L(sc.lights[is.area_light], is.n, wo) : sp1(0.0f);
+                L = L + beta * le;
             }
-            if (cls != 0u) {  // k_sort guarantees PF_HAS_RAY and a hit for classes >= 1
-                uint32_t bounces = flags >> PF_BOUNCES_SHIFT;
-                bool specular_bounce = (flags & PF_SPECULAR_BOUNCE) != 0;
-                const float4 hit = st_hit;
-                int prim = __float_as_int(hit.x);
-                if (prim >= 0) {
-                    n_vertices++;
-                    const float4 rd4 = st_rd, b4 = st_beta;
-                    V3 rd = mk3(rd4.x, rd4.y, rd4.z);
-                    Sp beta = mksp(b4.x, b4.y, b4.z);
-                    float eta_scale = b4.w;
-                    V3 wo = -rd;
-                    V3 wo_nee = wo;  // isect.wo: what estimate_direct evaluates the BSDF with (differs for a transformed instance hit)
-                    Isect is = INST ? hit_interaction(sc, rp.instancing, (uint32_t)prim, hit.y, hit.z, hit.w, ps.hit_inst[slot], rd, wo_nee)
-                                              : tri_interaction(sc, (uint32_t)prim, hit.y, hit.z, hit.w);
-                    if (bounces == 0 || specular_bounce) {
-                        // `l += beta * isect.le(&-ray.d)` (path.rs:97-100) also for a surface that emits nothing: le() is then black (interaction.rs:475-483),
-                        // and beta * 0 is NaN when a degenerate BSDF value has made a component of beta infinite.  (The reference asserts on an infinite
-                        // beta.y() right after the update, path.rs:158-171, so it aborts before it gets here; the oracle restates the arithmetic without
-                        // the asserts, and this statement keeps the two restatements equal there too: the sample ends as NaN and k_resolve's has_nans()
-                        // drops it -- tests/test_emu_kernels.py::test_randomised_materials_and_settings.)
-                        const Sp le = is.area_light >= 0 ? light_L(sc.lights[is.area_light], is.n, wo) : sp1(0.0f);
-                        L = L + beta * le;
+            if (bounces < rp.max_depth) {
+                if (is.material == 0xffffffffu) {  // null BSDF: pass through, bounce not counted (path.rs:109-116)
+                    V3 o = offset_ray_origin(is.p, is.p_error, is.n, rd);
+                    ext0 = make_float4(o.x, o.y, o.z, inf);
+                    ext1 = make_float4(rd.x, rd.y, rd.z, __uint_as_float(slot | (RAY_EXTEND << 30)));
+                    emit_ext = true;
+                    out_flags = (flags & ~0xffu) | (flags & PF_SPECULAR_BOUNCE) | PF_HAS_RAY;
+                } else {
+                    BsdfFrame B;
+                    B.mat = sc.materials + is.material;
+                    if (SPEC == 0 && (B.mat->cls & PB_MAT_TEXTURED)) {
+                        if (B.mat->cls & PB_MAT_BUMPED) {  // the bump-mapped shading frame of this hit (k_texture)
+                            const float4 f0 = ps.slot_frame[2 * (size_t)slot], f1 = ps.slot_frame[2 * (size_t)slot + 1];
+                            is.ns = mk3(f0.x, f0.y, f0.z);
+                            is.sh_dpdu = mk3(f1.x, f1.y, f1.z);  // the frame below is built from these two
+                        }
+                        B.mat = ps.slot_mat + slot;  // lobes of this hit, compiled by k_texture
                     }
-                    if (bounces < rp.max_depth) {
-                        if (is.material == 0xffffffffu) {  // null BSDF: pass through, bounce not counted (path.rs:109-116)
-                            V3 o = offset_ray_origin(is.p, is.p_error, is.n, rd);
-                            ext0 = make_float4(o.x, o.y, o.z, inf);
-                            ext1 = make_float4(rd.x, rd.y, rd.z, __uint_as_float(slot | (RAY_EXTEND << 30)));
-                            emit_ext = true;
-                            out_flags = (flags & ~0xffu) | (flags & PF_SPECULAR_BOUNCE) | PF_HAS_RAY;
-                        } else {
-                            BsdfFrame B;
-                            B.mat = sc.materials + is.material;
-                            if (SPEC == 0 && (B.mat->cls & PB_MAT_TEXTURED)) {
-                                if (B.mat->cls & PB_MAT_BUMPED) {  // the bump-mapped shading frame of this hit (k_texture)
-                                    const float4 f0 = ps.slot_frame[2 * (size_t)slot], f1 = ps.slot_frame[2 * (size_t)slot + 1];
-                                    is.ns = mk3(f0.x, f0.y, f0.z);
-                                    is.sh_dpdu = mk3(f1.x, f1.y, f1.z);  // the frame below is built from these two
-                                }
-                                B.mat = ps.slot_mat + slot;  // lobes of this hit, compiled by k_texture
-                            }
-                            B.ns = is.ns;
-                            B.ng = is.n;
-                            B.ss = norm3(is.sh_dpdu);
-                            B.ts = cross3(is.ns, B.ss);
-                            const uint2 si = st_sobol;
-                            SobolT sob;
-                            sob.nib = tab;
-                            sob.ds = tab_stride;
-                            sob.n_chunks = n_chunks;
-                            sob.index = ((uint64_t)si.y << 32) | si.x;
-                            sob.dim = st_dim;
-                            sob.overflow = false;
-                            uint32_t nee_flags = 0;
-                            if (SPEC >= 1 ? pb_spec_has_nonspecular(SPEC) : (B.mat->nonspecular > 0)) {
-                                // uniform_sample_one_light (integrator.rs:359-403); its result is added as
-                                // L += beta * Ld right here unless rays have to be traced first
-                                Sp ld_now = sp1(0.0f);
-                                const int nl = grid.n_lights;
-                                if (nl > 0) {
-                                    const size_t v = (rp.light_strategy == 2u) ? grid.row_of(light_voxel(sc, grid, is.p)) : (size_t)0;
-                                    float choice_pdf;
-                                    // light choice, u_light, u_scattering: five consecutive dimensions in one pass
-                                    float u5[5];
-                                    if (HALTON) {
+                    B.ns = is.ns;
+                    B.ng = is.n;
+                    B.ss = norm3(is.sh_dpdu);
+                    B.ts = cross3(is.ns, B.ss);
+                    const uint2 si = st_sobol;
+                    SobolT sob;
+                    sob.nib = tab;
+                    sob.ds = tab_stride;
+                    sob.n_chunks = n_chunks;
+                    sob.index = ((uint64_t)si.y << 32) | si.x;
+                    sob.dim = st_dim;
+                    sob.overflow = false;
+                    uint32_t nee_flags = 0;
+                    if (SPEC >= 1 ? pb_spec_has_nonspecular(SPEC) : (B.mat->nonspecular > 0)) {
+                        // uniform_sample_one_light (integrator.rs:359-403); its result is added as
+                        // L += beta * Ld right here unless rays have to be traced first
+                        Sp ld_now = sp1(0.0f);
+                        const int nl = grid.n_lights;
+                        if (nl > 0) {
+                            const size_t v = (rp.light_strategy == 2u) ? grid.row_of(light_voxel(sc, grid, is.p)) : (size_t)0;
+                            float choice_pdf;
+                            // light choice, u_light, u_scattering: five consecutive dimensions in one pass
+                            float u5[5];
+                            if (HALTON) {
 #pragma unroll
-                                        for (int k = 0; k < 5; ++k) u5[k] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim + (uint32_t)k, (uint32_t)(PB_HALTON_DIMS - 1)));
-                                    } else sobolT_fill<5>(sob, u5);
-                                    const float u_choice = sobolT_take<HALTON>(sob, 1) ? u5[0] : 0.0f;
-                                    int light_num = sample_discrete(grid.func + v * nl, grid.cdf + v * (nl + 1), grid.func_int[v], nl,
-                                                                    u_choice, choice_pdf);
-                                    if (choice_pdf != 0.0f) {
-                                        float2 u_light = make_float2(0.0f, 0.0f), u_scat = make_float2(0.0f, 0.0f);
-                                        if (sobolT_take<HALTON>(sob, 2)) u_light = make_float2(u5[1], u5[2]);
-                                        if (sobolT_take<HALTON>(sob, 2)) u_scat = make_float2(u5[3], u5[4]);
-                                        const DLight& light = sc.lights[light_num];
-                                        // estimate_direct (integrator.rs:406-570): light-sampling strategy
-                                        V3 wi = mk3(0.0f, 0.0f, 0.0f);
-                                        float light_pdf = 0.0f, scattering_pdf = 0.0f, mis_w = 0.0f;
-                                        Sp a = sp1(0.0f);
-                                        LightSample ls;
-                                        Sp li = light_sample_li<AREA_ONLY>(sc, light, is.p, u_light, wi, light_pdf, ls);
-                                        if (light_pdf > 0.0f && !is_black(li)) {
-                                            Sp f = bsdf_f<SPEC>(B, wo_nee, wi, NONSPEC) * sp1(absdot3(wi, is.ns));
-                                            scattering_pdf = bsdf_pdf<SPEC>(B, wo_nee, wi, NONSPEC);
-                                            if (!is_black(f)) {
-                                                // VisibilityTester::unoccluded -> spawn_ray_to (interaction.rs:81-94)
-                                                V3 origin = offset_ray_origin(is.p, is.p_error, is.n, ls.p - is.p);
-                                                V3 target = offset_ray_origin(ls.p, ls.p_error, ls.n, origin - ls.p);
-                                                V3 sd = target - origin;
-                                                if (!AREA_ONLY && light_is_delta(light)) a = f * li / light_pdf;  // is_delta_light: no MIS
-                                                else {
-                                                    float w = power_heuristic(light_pdf, scattering_pdf);
-                                                    a = f * li * sp1(w) / light_pdf;
-                                                }
-                                                sh0 = make_float4(origin.x, origin.y, origin.z, 1.0f - PB_SHADOW_EPSILON);
-                                                sh1 = make_float4(sd.x, sd.y, sd.z, __uint_as_float(slot | (RAY_SHADOW << 30)));
-                                                emit_sh = true;
-                                                nee_flags |= PF_HAS_SHADOW;
-                                            }
+                                for (int k = 0; k < 5; ++k) u5[k] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim + (uint32_t)k, (uint32_t)(PB_HALTON_DIMS - 1)));
+                            } else sobolT_fill<5>(sob, u5);
+                            const float u_choice = sobolT_take<HALTON>(sob, 1) ? u5[0] : 0.0f;
+                            int light_num = sample_discrete(grid.func + v * nl, grid.cdf + v * (nl + 1), grid.func_int[v], nl,
+                                                            u_choice, choice_pdf);
+                            if (choice_pdf != 0.0f) {
+                                float2 u_light = make_float2(0.0f, 0.0f), u_scat = make_float2(0.0f, 0.0f);
+                                if (sobolT_take<HALTON>(sob, 2)) u_light = make_float2(u5[1], u5[2]);
+                                if (sobolT_take<HALTON>(sob, 2)) u_scat = make_float2(u5[3], u5[4]);
+                                const DLight& light = sc.lights[light_num];
+                                // estimate_direct (integrator.rs:406-570): light-sampling strategy
+                                V3 wi = mk3(0.0f, 0.0f, 0.0f);
+                                float light_pdf = 0.0f, scattering_pdf = 0.0f, mis_w = 0.0f;
+                                Sp a = sp1(0.0f);
+                                LightSample ls;
+                                Sp li = light_sample_li<AREA_ONLY>(sc, light, is.p, u_light, wi, light_pdf, ls);
+                                if (light_pdf > 0.0f && !is_black(li)) {
+                                    Sp f = bsdf_f<SPEC>(B, wo_nee, wi, NONSPEC) * sp1(absdot3(wi, is.ns));
+                                    scattering_pdf = bsdf_pdf<SPEC>(B, wo_nee, wi, NONSPEC);
+                                    if (!is_black(f)) {
+                                        // VisibilityTester::unoccluded -> spawn_ray_to (interaction.rs:81-94)
+                                        V3 origin = offset_ray_origin(is.p, is.p_error, is.n, ls.p - is.p);
+                                        V3 target = offset_ray_origin(ls.p, ls.p_error, ls.n, origin - ls.p);
+                                        V3 sd = target - origin;
+                                        if (!AREA_ONLY && light_is_delta(light)) a = f * li / light_pdf;  // is_delta_light: no MIS
+                                        else {
+                                            float w = power_heuristic(light_pdf, scattering_pdf);
+                                            a = f * li * sp1(w) / light_pdf;
                                         }
-                                        // BSDF-sampling strategy (skipped for delta lights, integrator.rs:480); `wi` is shared
-                                        // with the light strategy as in the reference, sampled_type = 0 in (quirk Q8)
-                                        int st = 0;
-                                        Sp f2 = sp1(0.0f);
-                                        if (AREA_ONLY || !light_is_delta(light)) {
-                                            f2 = bsdf_sample_f<SPEC>(B, wo_nee, wi, u_scat, scattering_pdf, NONSPEC, st);
-                                            f2 = f2 * sp1(absdot3(wi, is.ns));
-                                        }
-                                        if (!is_black(f2) && scattering_pdf > 0.0f) {
-                                            V3 mo = offset_ray_origin(is.p, is.p_error, is.n, wi);  // it.spawn_ray(wi)
-                                            if (AREA_ONLY || light.kind == 0u) n_light_tests++;  // Triangle::intersect inside pdf_li (area lights only)
-                                            float lp = light_pdf_li<AREA_ONLY>(sc, light, is.p, mo, wi);
-                                            if (lp != 0.0f) {
-                                                mis_w = power_heuristic(scattering_pdf, lp);
-                                                mis0 = make_float4(mo.x, mo.y, mo.z, inf);
-                                                mis1 = make_float4(wi.x, wi.y, wi.z, __uint_as_float(slot | (RAY_MIS << 30)));
-                                                emit_mis = true;
-                                                ps.mis_d[slot] = make_float4(wi.x, wi.y, wi.z, __uint_as_float((uint32_t)light_num));
-                                                ps.mis_f[slot] = make_float4(f2.r, f2.g, f2.b, scattering_pdf);
-                                                nee_flags |= PF_HAS_MIS;
-                                            }
-                                        }
-                                        if (nee_flags) {
-                                            ps.ld_light[slot] = make_float4(a.r, a.g, a.b, mis_w);
-                                            ps.nee_beta[slot] = make_float4(beta.r, beta.g, beta.b, choice_pdf);
-                                        } else ld_now = spdiv0(sp1(0.0f), choice_pdf);
+                                        sh0 = make_float4(origin.x, origin.y, origin.z, 1.0f - PB_SHADOW_EPSILON);
+                                        sh1 = make_float4(sd.x, sd.y, sd.z, __uint_as_float(slot | (RAY_SHADOW << 30)));
+                                        emit_sh = true;
+                                        nee_flags |= PF_HAS_SHADOW;
                                     }
                                 }
-                                if (!nee_flags) L = L + beta * ld_now;
+                                // BSDF-sampling strategy (skipped for delta lights, integrator.rs:480); `wi` is shared
+                                // with the light strategy as in the reference, sampled_type = 0 in (quirk Q8)
+                                int st = 0;
+                                Sp f2 = sp1(0.0f);
+                                if (AREA_ONLY || !light_is_delta(light)) {
+                                    f2 = bsdf_sample_f<SPEC>(B, wo_nee, wi, u_scat, scattering_pdf, NONSPEC, st);
+                                    f2 = f2 * sp1(absdot3(wi, is.ns));
+                                }
+                                if (!is_black(f2) && scattering_pdf > 0.0f) {
+                                    V3 mo = offset_ray_origin(is.p, is.p_error, is.n, wi);  // it.spawn_ray(wi)
+                                    if (AREA_ONLY || light.kind == 0u) n_light_tests++;  // Triangle::intersect inside pdf_li (area lights only)
+                                    float lp = light_pdf_li<AREA_ONLY>(sc, light, is.p, mo, wi);
+                                    if (lp != 0.0f) {
+                                        mis_w = power_heuristic(scattering_pdf, lp);
+                                        mis0 = make_float4(mo.x, mo.y, mo.z, inf);
+                                        mis1 = make_float4(wi.x, wi.y, wi.z, __uint_as_float(slot | (RAY_MIS << 30)));
+                                        emit_mis = true;
+                                        ps.mis_d[slot] = make_float4(wi.x, wi.y, wi.z, __uint_as_float((uint32_t)light_num));
+                                        ps.mis_f[slot] = make_float4(f2.r, f2.g, f2.b, scattering_pdf);
+                                        nee_flags |= PF_HAS_MIS;
+                                    }
+                                }
+                                if (nee_flags) {
+                                    ps.ld_light[slot] = make_float4(a.r, a.g, a.b, mis_w);
+                                    ps.nee_beta[slot] = make_float4(beta.r, beta.g, beta.b, choice_pdf);
+                                } else ld_now = spdiv0(sp1(0.0f), choice_pdf);
                             }
-                            // sample the BSDF for the next direction (path.rs:141-188)
-                            V3 wi = mk3(0.0f, 0.0f, 0.0f);
-                            float pdf = 0.0f;
-                            int st = 255;
-                            float u3[3];  // BSDF sample + the Russian-roulette dimension behind it
-                            if (HALTON) {
-                                u3[0] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim, (uint32_t)(PB_HALTON_DIMS - 1)));
-                                u3[1] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim + 1u, (uint32_t)(PB_HALTON_DIMS - 1)));
-                                u3[2] = 0.0f;  // the roulette dimension is drawn only when it is needed (below)
-                            } else sobolT_fill<3>(sob, u3);
-                            const float2 u_bsdf = sobolT_take<HALTON>(sob, 2) ? make_float2(u3[0], u3[1]) : make_float2(0.0f, 0.0f);
-                            Sp f = bsdf_sample_f<SPEC>(B, wo, wi, u_bsdf, pdf, BSDF_ALL, st);
-                            bool alive = !(is_black(f) || pdf == 0.0f);
-                            if (alive) {
-                                beta = beta * ((f * absdot3(wi, is.ns)) / pdf);
-                                specular_bounce = (st & BSDF_SPECULAR) != 0;
-                                if ((st & BSDF_SPECULAR) && (st & BSDF_TRANSMISSION)) {
-                                    float eta = B.mat->eta;
-                                    if (dot3(wo, is.n) > 0.0f) eta_scale *= eta * eta;
-                                    else eta_scale *= 1.0f / (eta * eta);
-                                }
-                                V3 o = offset_ray_origin(is.p, is.p_error, is.n, wi);
-                                // Russian roulette (path.rs:251-262)
-                                Sp rr_beta = beta * eta_scale;
-                                if (maxsp(rr_beta) < rp.rr_threshold && bounces > 3) {
-                                    float q = fmaxf(0.05f, 1.0f - maxsp(rr_beta));
-                                    if (HALTON) u3[2] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim, (uint32_t)(PB_HALTON_DIMS - 1)));
-                                    const float u_rr = sobolT_take<HALTON>(sob, 1) ? u3[2] : 0.0f;
-                                    if (u_rr < q) alive = false;
-                                    else beta = beta / (1.0f - q);
-                                }
-                                if (alive) {
-                                    ext0 = make_float4(o.x, o.y, o.z, inf);
-                                    ext1 = make_float4(wi.x, wi.y, wi.z, __uint_as_float(slot | (RAY_EXTEND << 30)));
-                                    emit_ext = true;
-                                    ps.ray_d[slot] = make_float4(wi.x, wi.y, wi.z, 0.0f);
-                                    ps.beta[slot] = make_float4(beta.r, beta.g, beta.b, eta_scale);
-                                    ps.dim[slot] = sob.dim;
-                                    out_flags = ((bounces + 1) << PF_BOUNCES_SHIFT) | (specular_bounce ? PF_SPECULAR_BOUNCE : 0u) | PF_HAS_RAY;
-                                }
-                            }
-                            out_flags |= nee_flags;
-                            if (sob.overflow) atomicOr(d_error, 1u);
+                        }
+                        if (!nee_flags) L = L + beta * ld_now;
+                    }
+                    // sample the BSDF for the next direction (path.rs:141-188)
+                    V3 wi = mk3(0.0f, 0.0f, 0.0f);
+                    float pdf = 0.0f;
+                    int st = 255;
+                    float u3[3];  // BSDF sample + the Russian-roulette dimension behind it
+                    if (HALTON) {
+                        u3[0] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim, (uint32_t)(PB_HALTON_DIMS - 1)));
+                        u3[1] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim + 1u, (uint32_t)(PB_HALTON_DIMS - 1)));
+                        u3[2] = 0.0f;  // the roulette dimension is drawn only when it is needed (below)
+                    } else sobolT_fill<3>(sob, u3);
+                    const float2 u_bsdf = sobolT_take<HALTON>(sob, 2) ? make_float2(u3[0], u3[1]) : make_float2(0.0f, 0.0f);
+                    Sp f = bsdf_sample_f<SPEC>(B, wo, wi, u_bsdf, pdf, BSDF_ALL, st);
+                    bool alive = !(is_black(f) || pdf == 0.0f);
+                    if (alive) {
+                        beta = beta * ((f * absdot3(wi, is.ns)) / pdf);
+                        specular_bounce = (st & BSDF_SPECULAR) != 0;
+                        if ((st & BSDF_SPECULAR) && (st & BSDF_TRANSMISSION)) {
+                            float eta = B.mat->eta;
+                            if (dot3(wo, is.n) > 0.0f) eta_scale *= eta * eta;
+                            else eta_scale *= 1.0f / (eta * eta);
+                        }
+                        V3 o = offset_ray_origin(is.p, is.p_error, is.n, wi);
+                        // Russian roulette (path.rs:251-262)
+                        Sp rr_beta = beta * eta_scale;
+                        if (maxsp(rr_beta) < rp.rr_threshold && bounces > 3) {
+                            float q = fmaxf(0.05f, 1.0f - maxsp(rr_beta));
+                            if (HALTON) u3[2] = halton_scrambled(rp, (uint32_t)sob.index, min(sob.dim, (uint32_t)(PB_HALTON_DIMS - 1)));
+                            const float u_rr = sobolT_take<HALTON>(sob, 1) ? u3[2] : 0.0f;
+                            if (u_rr < q) alive = false;
+                            else beta = beta / (1.0f - q);
+                        }
+                        if (alive) {
+                            ext0 = make_float4(o.x, o.y, o.z, inf);
+                            ext1 = make_float4(wi.x, wi.y, wi.z, __uint_as_float(slot | (RAY_EXTEND << 30)));
+                            emit_ext = true;
+                            ps.ray_d[slot] = make_float4(wi.x, wi.y, wi.z, 0.0f);
+                            ps.beta[slot] = make_float4(beta.r, beta.g, beta.b, eta_scale);
+                            ps.dim[slot] = sob.dim;
+                            out_flags = ((bounces + 1) << PF_BOUNCES_SHIFT) | (specular_bounce ? PF_SPECULAR_BOUNCE : 0u) | PF_HAS_RAY;
                         }
                     }
+                    out_flags |= nee_flags;
+                    if (sob.overflow) atomicOr(d_error, 1u);
                 }
             }
             ps.L[slot] = make_float4(L.r, L.g, L.b, __uint_as_float(out_flags));

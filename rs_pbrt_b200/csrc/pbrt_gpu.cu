@@ -1766,14 +1766,18 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 shade_plan.push_back({0, c, e});
                 c = e;
             }
-            // class 0 ("nothing to shade": only a pending next-event estimate to resolve) and, when no material has class 1, the
-            // null-material hits that k_sort files under class 1: folded into the Lambert launch when nothing lies between, else a launch
-            // of their own (the cheapest instantiation: no BSDF is touched)
+            // when no material has class 1, the null-material hits that k_sort files under class 1 (a shape without a material, or a
+            // moved instance under quirk Q7): folded into the Lambert launch when nothing lies between, else a launch of their own (the
+            // cheapest instantiation: no BSDF is touched).  An otherwise empty plan keeps that launch too: k_shade resets the counters
+            // the next iteration fills.
             const uint32_t lam = 1 + LOBE_LAMBERT;
-            bool folded = false;
-            if ((covered & (1u << lam)) && (mask & ((1u << lam) - 2u)) == 0u)
-                for (ShadeLaunch& l : shade_plan) if (l.spec == (int)lam) { l.lo = 0; folded = true; }
-            if (!folded) shade_plan.insert(shade_plan.begin(), ShadeLaunch{shade_spec ? (int)lam : 0, 0u, (mask & 2u) ? 1u : 2u});
+            const bool null_hits = sc->has_null_material || (plan_instanced && p->instancing == PBRT_INSTANCING_REFERENCE);
+            if (!(mask & 2u) && (null_hits || shade_plan.empty())) {
+                bool folded = false;
+                if ((covered & (1u << lam)) && (mask & ((1u << lam) - 4u)) == 0u)
+                    for (ShadeLaunch& l : shade_plan) if (l.spec == (int)lam) { l.lo = 1; folded = true; }
+                if (!folded) shade_plan.insert(shade_plan.begin(), ShadeLaunch{shade_spec ? (int)lam : 0, 1u, 2u});
+            }
         }
         // Two batches in flight on two streams: k_trace is issue bound, k_shade latency bound, so letting one batch
         // trace while the other shades fills the SMs better than either alone.  Disabled for the roofline timing pass
