@@ -14,7 +14,7 @@ import pytest
 ROOT = Path(__file__).resolve().parent.parent
 pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="needs g++")
 
-FILES = ["test_gpu_parity_cornell.py", "test_gpu_parity_halton.py", "test_gpu_parity_lights.py", "test_gpu_parity_materials.py", "test_gpu_parity_siblings.py"]
+FILES = ["test_gpu_closed_forms.py", "test_gpu_parity_cornell.py", "test_gpu_parity_halton.py", "test_gpu_parity_lights.py", "test_gpu_parity_materials.py", "test_gpu_parity_siblings.py"]
 
 
 @pytest.mark.parametrize("name", FILES)
