@@ -21,7 +21,8 @@
  * ABI versions (pbrt_gpu_abi_version): 1 = area lights, Sobol', path integrator; 2 = all light kinds, Halton, ao, object instances;
  * 3 = image textures (PbrtTexture, PbrtMaterial.tex / bump, PbrtSceneDesc.textures), PbrtLight.n_samples, the directlighting and
  * whitted integrators (PbrtRenderParams.direct_strategy); 4 = PbrtStats.shade_slots / shaded_vertices, tile-interleaved rendering
- * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi).  Structs only ever grow at their end
+ * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi); within 4, the animated camera
+ * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed).  Structs only ever grow at their end
  * within a version step, and a zero-initialised new field means "as before".
  */
 #ifndef PBRT_GPU_H
@@ -228,7 +229,8 @@ typedef struct PbrtLight {
 } PbrtLight;
 
 /* PerspectiveCamera (src/cameras/perspective.rs:23-43); row-major 4x4, m[r][c] = a[4*r+c].
- * camera_to_world must be static (start_transform); animated => PBRT_E_UNSUPPORTED upstream. */
+ * camera_to_world is the camera's start transform; an animated camera also hands its AnimatedTransform to
+ * pbrt_gpu_scene_create_motion (below). */
 typedef struct PbrtCamera {
     float raster_to_camera[16];
     float camera_to_world[16];
@@ -329,6 +331,31 @@ typedef struct PbrtScene PbrtScene;
 /* Upload a flattened scene to `device` (CUDA ordinal).  Replaces the per-tile
  * scene access of integrator.rs:107-205. */
 int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out);
+
+/* ---- motion blur ---------------------------------------------------------------------------------------------------------------
+ * A two-keyframe AnimatedTransform (src/core/transform.rs:893-940): the inputs of AnimatedTransform::new, i.e. the start and end
+ * Transforms (m and m_inv of each, row-major) and TransformTimes.  The library restates AnimatedTransform::new (decompose, the
+ * shortest-path flip of the end rotation) once at scene creation and AnimatedTransform::interpolate on the device. */
+typedef struct PbrtAnimatedTransform {
+    float start[16], start_inv[16];
+    float end[16], end_inv[16];
+    float start_time, end_time;
+} PbrtAnimatedTransform;
+/* camera: the camera's camera_to_world (api.rs:497-502), NULL = static.  Its start must equal PbrtSceneDesc.camera.camera_to_world.
+ *   Each camera sample is traced at ray.time = lerp(sample.time, shutter_open, shutter_close) (perspective.rs:226) through
+ *   camera_to_world interpolated at that time (AnimatedTransform::transform_ray, transform.rs:2114-2124).
+ * instances: NULL, or one entry per PbrtSceneDesc.instances (api.rs:3093-3101), whose start equals PbrtInstance.m / m_inv.  An
+ *   instance whose keyframes differ is PBRT_E_UNSUPPORTED in this version: animated object instances and animated shapes stay on the
+ *   caller's CPU loop.
+ * Keyframes or times that are not finite are PBRT_E_UNSUPPORTED; a camera keyframe whose m_inv is not the inverse of its m (up to f32
+ * rounding) is PBRT_E_INVALID. */
+typedef struct PbrtMotionDesc {
+    const PbrtAnimatedTransform* camera;
+    const PbrtAnimatedTransform* instances;
+} PbrtMotionDesc;
+/* pbrt_gpu_scene_create with a motion description; motion == NULL is pbrt_gpu_scene_create.  A caller detects motion blur support
+ * by this symbol. */
+int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out);
 void pbrt_gpu_scene_destroy(PbrtScene* scene);
 /* Optional (ABI v4): page-lock a host array the caller owns -- nodes, tris, a mesh's p / n / s / uv -- so that pbrt_gpu_scene_create
  * DMAs it where it lies (cudaHostRegister, portable across devices); an array that is not pinned is copied through the library's
@@ -398,6 +425,9 @@ int pbrt_gpu_kat_sincos(int device, uint32_t n, const float* x, float* sin_out, 
 int pbrt_gpu_kat_acos_atan2(int device, uint32_t n, const float* x, const float* y, float* acos_out, float* atan2_out);
 /* Same for log2(x[i]) (glibc's log2f; MIPMap level selection). */
 int pbrt_gpu_kat_log2(int device, uint32_t n, const float* x, float* log2_out);
+/* Known-answer hook for motion blur: AnimatedTransform::new of *at on the host, then AnimatedTransform::interpolate on the device at
+ * n times, writing 16 floats of m and 16 of m_inv per time (row-major).  Not part of the render path. */
+int pbrt_gpu_kat_animated_interpolate(int device, const PbrtAnimatedTransform* at, uint32_t n, const float* times, float* m_out, float* m_inv_out);
 
 #ifdef __cplusplus
 }

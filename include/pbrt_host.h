@@ -5,6 +5,7 @@
  * written in C++ and mirrors the reference's own call sequence for the path:
  *   pbrt_shape / pbrt_area_light_source      src/core/api.rs:2792-2870   -> pbrt_host_add_trianglemesh
  *   pbrt_look_at / make_camera               src/core/api.rs:486-514, src/cameras/perspective.rs:46-185
+ *   pbrt_transform_times / animated camera   src/core/api.rs:497-502,2525-2529 -> pbrt_host_camera_motion
  *   make_film / make_filter                  src/core/film.rs:176-262, src/filters
  *   make_sampler ("sobol")                   src/samplers/sobol.rs:37-108
  *   make_integrator ("path")                 src/core/api.rs:285-321
@@ -82,6 +83,12 @@ int pbrt_host_add_light_distant(PbrtHost* h, const float from[3], const float to
 int pbrt_host_add_light_infinite(PbrtHost* h, const float L[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
                                  const float* light_to_world, const float* world_to_light);
 int pbrt_host_look_at(PbrtHost* h, const float eye[3], const float look[3], const float up[3]);
+/* TransformTimes start end (api.rs:2525-2529; defaults 0 and 1): the times of the start and end keyframes of every AnimatedTransform. */
+int pbrt_host_transform_times(PbrtHost* h, float start, float end);
+/* The camera's end keyframe (`ActiveTransform EndTime` before the Camera directive): camera_to_world at the end time, row-major 4x4;
+ * the start keyframe is the one pbrt_host_look_at set.  NULL = a static camera again.  make_camera then builds the camera's
+ * AnimatedTransform (api.rs:497-502); pbrt_host_motion_desc hands it to pbrt_gpu_scene_create_motion. */
+int pbrt_host_camera_motion(PbrtHost* h, const float* camera_to_world_end);
 /* Film "image": crop = {x0,x1,y0,y1} in [0,1] or NULL; filter_name "box" | "gaussian" | "triangle" (xwidth/ywidth = radius) */
 int pbrt_host_film(PbrtHost* h, int xres, int yres, const float* crop, const char* filter_name, float xwidth, float ywidth, float filter_alpha,
                    float max_sample_luminance);
@@ -105,6 +112,8 @@ int pbrt_host_world_end(PbrtHost* h, uint32_t max_prims_in_node, int n_threads);
 
 const PbrtSceneDesc* pbrt_host_scene_desc(const PbrtHost* h);
 const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h);
+/* The motion description of the built scene, NULL when nothing in it is animated. */
+const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h);
 
 /* Integrator::render(scene, num_threads): uploads the scene, renders pixel_rect (NULL = whole sample bounds) on `device`
  * through pbrt_gpu_render, and merges the result into the Film like merge_film_tile. */

@@ -75,6 +75,15 @@ class PbrtSceneDesc(C.Structure):
                 ("textures", C.POINTER(PbrtTexture)), ("n_textures", C.c_uint32)]
 
 
+class PbrtAnimatedTransform(C.Structure):
+    _fields_ = [("start", C.c_float * 16), ("start_inv", C.c_float * 16), ("end", C.c_float * 16), ("end_inv", C.c_float * 16),
+                ("start_time", C.c_float), ("end_time", C.c_float)]
+
+
+class PbrtMotionDesc(C.Structure):
+    _fields_ = [("camera", C.POINTER(PbrtAnimatedTransform)), ("instances", C.POINTER(PbrtAnimatedTransform))]
+
+
 class PbrtRenderParams(C.Structure):
     _fields_ = [("sample_bounds", C.c_int32 * 4), ("cropped_pixel_bounds", C.c_int32 * 4), ("pixel_bounds", C.c_int32 * 4),
                 ("filter_radius", C.c_float * 2), ("filter_table", C.c_float * 256), ("max_sample_luminance", C.c_float),
@@ -95,9 +104,10 @@ class PbrtStats(C.Structure):
 
 GPU_SYMBOLS = ["pbrt_gpu_scene_create", "pbrt_gpu_scene_destroy", "pbrt_gpu_scene_bytes", "pbrt_gpu_render", "pbrt_gpu_render_device", "pbrt_gpu_render_samples",
                "pbrt_gpu_render_tiles_device", "pbrt_gpu_render_multi", "pbrt_gpu_host_register", "pbrt_gpu_host_unregister",
-               "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2"]
+               "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2",
+               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate"]
 HOST_SYMBOLS = ["pbrt_host_new", "pbrt_host_free", "pbrt_host_last_error", "pbrt_host_add_material", "pbrt_host_add_material_mix", "pbrt_host_add_trianglemesh",
-                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_look_at", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
+                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
                 "pbrt_host_integrator_path", "pbrt_host_world_end", "pbrt_host_scene_desc", "pbrt_host_render_params", "pbrt_host_render",
                 "pbrt_host_film_rgbw", "pbrt_host_film_clear", "pbrt_host_film_add_rgbw", "pbrt_host_film_rgb", "pbrt_host_write_image",
                 "pbrt_host_bvh_build"]
@@ -125,6 +135,8 @@ def bind(L):
     fp, ip, u8p, u32p = C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_uint8), C.POINTER(C.c_uint32)
     vp = C.c_void_p
     L.pbrt_gpu_scene_create.argtypes = [C.POINTER(PbrtSceneDesc), C.c_int, C.POINTER(vp)]
+    L.pbrt_gpu_scene_create_motion.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.c_int, C.POINTER(vp)]
+    L.pbrt_gpu_kat_animated_interpolate.argtypes = [C.c_int, C.POINTER(PbrtAnimatedTransform), C.c_uint32, fp, fp, fp]
     L.pbrt_gpu_scene_destroy.argtypes = [vp]
     L.pbrt_gpu_scene_destroy.restype = None
     L.pbrt_gpu_scene_bytes.argtypes = [vp]
@@ -155,6 +167,10 @@ def bind(L):
     L.pbrt_host_add_light_distant.argtypes = [vp, fp, fp, fp, fp]
     L.pbrt_host_add_light_infinite.argtypes = [vp, fp, fp, fp, C.c_uint32, C.c_uint32, fp, fp]
     L.pbrt_host_look_at.argtypes = [vp, fp, fp, fp]
+    L.pbrt_host_transform_times.argtypes = [vp, C.c_float, C.c_float]
+    L.pbrt_host_camera_motion.argtypes = [vp, fp]
+    L.pbrt_host_motion_desc.argtypes = [vp]
+    L.pbrt_host_motion_desc.restype = C.POINTER(PbrtMotionDesc)
     L.pbrt_host_film.argtypes = [vp, C.c_int, C.c_int, fp, C.c_char_p, C.c_float, C.c_float, C.c_float, C.c_float]
     L.pbrt_host_camera_perspective.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, fp]
     L.pbrt_host_sampler_sobol.argtypes = [vp, C.c_int]

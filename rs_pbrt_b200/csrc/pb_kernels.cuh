@@ -18,6 +18,7 @@
 #include "pb_sobol.cuh"
 #include "pb_texture.cuh"
 #include "pb_material.cuh"
+#include "pb_motion.cuh"
 
 namespace pb {
 
@@ -100,10 +101,12 @@ struct BatchInfo {
 
 // -----------------------------------------------------------------------------------------------
 // k_raygen: integrator.rs:123-144, sampler.rs:85-95, sobol.rs:110-138, perspective.rs:190-280
+// CAM_MOTION: the camera is animated (cam_mo); a static camera's instantiation never reads cam_mo.
+template <bool CAM_MOTION>
 __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps, BatchInfo bi, const uint32_t* __restrict__ nib, uint32_t n_chunks,
                                                const uint64_t* __restrict__ vdc, const uint64_t* __restrict__ vdci, uint32_t* __restrict__ queue,
                                                uint32_t* __restrict__ d_count, float4* __restrict__ rays, uint32_t* __restrict__ d_nrays,
-                                               DCounters* cnt) {
+                                               DCounters* cnt, const DMotion cam_mo) {
     __shared__ uint64_t s_vdc[52], s_vdci[52];
     if (threadIdx.x < 52) {
         uint32_t m = rp.log2_res;
@@ -163,6 +166,11 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
             if (wp != 1.0f) { float inv = 1.0f / wp; pc = mk3(inv * xp, inv * yp, inv * zp); }
             V3 o = mk3(0.0f, 0.0f, 0.0f), d = norm3(pc);
             (void)time;  // ray.time only selects an animated transform; static cameras ignore it
+            float c2w_t[16];
+            if (CAM_MOTION) {  // AnimatedTransform::transform_ray (transform.rs:2114-2124) at ray.time = lerp(sample.time, shutter) (perspective.rs:226)
+                float c2w_inv_t[16];
+                motion_interpolate(cam_mo, lerpf(time, sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
+            }
             if (sc.lens_radius > 0.0f) {
                 float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
                 pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
@@ -172,7 +180,7 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
                 d = norm3(p_focus - o);
             }
             // camera -> world (Transform::transform_ray transform.rs:538-550, with origin error offset :662-708)
-            const float* c = sc.camera_to_world;
+            const float* c = CAM_MOTION ? c2w_t : sc.camera_to_world;
             x = o.x; y = o.y; z = o.z;
             V3 ow = mk3(c[0] * x + c[1] * y + c[2] * z + c[3], c[4] * x + c[5] * y + c[6] * z + c[7], c[8] * x + c[9] * y + c[10] * z + c[11]);
             float wpc = c[12] * x + c[13] * y + c[14] * z + c[15];
@@ -1200,6 +1208,11 @@ __global__ void __launch_bounds__(256) k_film_sum_peers(float4* __restrict__ dst
     }
 }
 
+// known-answer hook for AnimatedTransform::interpolate (pbrt_gpu_kat_animated_interpolate)
+__global__ void k_kat_motion(const DMotion mo, const float* __restrict__ t, uint32_t n, float* __restrict__ m, float* __restrict__ m_inv) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) motion_interpolate(mo, t[i], m + 16 * (size_t)i, m_inv + 16 * (size_t)i);
+}
 // known-answer hook for the device sin/cos (pbrt_gpu_kat_sincos)
 __global__ void k_kat_sincos(const float* __restrict__ x, uint32_t n, float* __restrict__ s, float* __restrict__ c) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

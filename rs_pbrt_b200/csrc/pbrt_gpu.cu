@@ -538,6 +538,8 @@ struct PbrtScene {
     DevBuf<float> ewa_lut;
     std::vector<Sp> h_env_power;  // per light: lmap.lookup((.5,.5), .5) for InfiniteAreaLight::power
     bool has_null_material = false;
+    bool cam_motion = false;  // the camera is animated: k_raygen<true> interpolates cam_mo at each sample's time
+    DMotion cam_mo;
     bool area_only = true;  // every light is a DiffuseAreaLight: k_shade<true> has the other kinds compiled out
     uint32_t class_mask = 0;  // bit c: some material has shading class c (1..8: a single lobe of kind c - 1; 9: Lambert + microfacet reflection; 10..15: everything else)
     size_t upload_bytes = 0;
@@ -1305,6 +1307,59 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     return PBRT_OK;
 }
 
+static bool finite_keyframes(const PbrtAnimatedTransform& a) {
+    bool ok = std::isfinite(a.start_time) && std::isfinite(a.end_time);
+    for (int k = 0; k < 16; ++k)
+        ok = ok && std::isfinite(a.start[k]) && std::isfinite(a.start_inv[k]) && std::isfinite(a.end[k]) && std::isfinite(a.end_inv[k]);
+    return ok;
+}
+
+// m_inv is the inverse of m up to f32 rounding: every element of m * m_inv (in f64) lies within 1e-4 of the sum of the magnitudes of
+// its terms of the identity's element.  A caller that hands over another matrix's inverse (or a transposed one) is caught here.
+static bool inverse_pair(const float* m, const float* m_inv) {
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j) {
+            double p = 0.0, mag = 0.0;
+            for (int k = 0; k < 4; ++k) { p += (double)m[4 * i + k] * m_inv[4 * k + j]; mag += std::fabs((double)m[4 * i + k] * m_inv[4 * k + j]); }
+            if (!(std::fabs(p - (i == j ? 1.0 : 0.0)) <= 1e-4 * mag + 1e-6)) return false;
+        }
+    return true;
+}
+
+int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out) {
+    if (!motion) return pbrt_gpu_scene_create(desc, device, out);
+    if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
+    *out = nullptr;
+    if (motion->instances) {
+        if (desc->n_instances && !desc->instances) return fail(PBRT_E_INVALID, "null instance array in scene description");
+        for (uint32_t i = 0; i < desc->n_instances; ++i) {
+            const PbrtAnimatedTransform& a = motion->instances[i];
+            if (!finite_keyframes(a)) return fail(PBRT_E_UNSUPPORTED, "instance keyframe matrix or time is not finite");
+            if (std::memcmp(a.start, desc->instances[i].m, 64) != 0 || std::memcmp(a.start_inv, desc->instances[i].m_inv, 64) != 0)
+                return fail(PBRT_E_INVALID, "an instance's start keyframe differs from PbrtInstance.m / m_inv");
+            for (int k = 0; k < 16; ++k)
+                if (a.start[k] != a.end[k] || a.start_inv[k] != a.end_inv[k])
+                    return fail(PBRT_E_UNSUPPORTED, "animated object instances are outside the GPU path");
+        }
+    }
+    DMotion cam_mo;
+    std::memset(&cam_mo, 0, sizeof cam_mo);
+    if (const PbrtAnimatedTransform* c = motion->camera) {
+        if (!finite_keyframes(*c)) return fail(PBRT_E_UNSUPPORTED, "camera keyframe matrix or time is not finite");
+        if (std::memcmp(c->start, desc->camera.camera_to_world, 64) != 0)
+            return fail(PBRT_E_INVALID, "the camera's start keyframe differs from PbrtCamera.camera_to_world");
+        if (!inverse_pair(c->start, c->start_inv) || !inverse_pair(c->end, c->end_inv))
+            return fail(PBRT_E_INVALID, "a camera keyframe's m_inv is not the inverse of its m");
+        motion_create(c->start, c->start_inv, c->start_time, c->end, c->end_inv, c->end_time, cam_mo);
+    }
+    const int rc = pbrt_gpu_scene_create(desc, device, out);
+    if (rc != PBRT_OK) return rc;
+    // a camera whose keyframes are equal takes the static kernels: interpolate() would hand back the start transform at every time
+    (*out)->cam_motion = cam_mo.actually_animated != 0;
+    (*out)->cam_mo = cam_mo;
+    return PBRT_OK;
+}
+
 int pbrt_gpu_host_register(const void* ptr, uint64_t bytes) {
     if (!ptr || !bytes) return fail(PBRT_E_INVALID, "null argument");
     cudaError_t e = cudaHostRegister(const_cast<void*>(ptr), (size_t)bytes, cudaHostRegisterPortable);
@@ -1597,8 +1652,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                k_raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, sc->nib.p, std::max(raygen_chunks, dd.n_chunks), sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count,
-                                                        X.rays.p, d_nrays, sc->counters.p);
+                const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+                raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, sc->nib.p, std::max(raygen_chunks, dd.n_chunks), sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count,
+                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo);
                 launches++;
                 // the recursion's length is decided on the device (the active word = camera samples that still need an iteration).  The
                 // host reads that word poll_lag() iterations late (see there: 0 by default, measured): with a lag of 1 iteration i + 1 is
@@ -1702,8 +1758,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                k_raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count, X.rays.p, d_nrays,
-                                                        sc->counters.p);
+                const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+                raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count, X.rays.p, d_nrays,
+                                                        sc->counters.p, sc->cam_mo);
                 launches++;
                 int rc = trace();
                 if (rc != PBRT_OK) return rc;
@@ -2088,8 +2145,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             // ray count, ray cursor, both sets of class counts (and the voxel requests): from here on the kernels reset them for each other
             CK(cudaMemsetAsync(V.d_nrays, 0, (5 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
             if (spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
-            k_raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays,
-                                                      sc->counters.p);
+            const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+            raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays,
+                                                      sc->counters.p, sc->cam_mo);
             launches++;
             return PBRT_OK;
         };
@@ -2497,6 +2555,27 @@ int pbrt_gpu_kat_acos_atan2(int device, uint32_t n, const float* x, const float*
     g_launches++;
     CK(cudaMemcpy(acos_out, da.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(atan2_out, dt.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return PBRT_OK;
+}
+
+// Known-answer hook: AnimatedTransform::new on the host (pb_motion.cuh), AnimatedTransform::interpolate on the device at n times.
+int pbrt_gpu_kat_animated_interpolate(int device, const PbrtAnimatedTransform* at, uint32_t n, const float* times, float* m_out, float* m_inv_out) {
+    if (!at || (n && (!times || !m_out || !m_inv_out))) return fail(PBRT_E_INVALID, "null argument");
+    int rc = check_device(device);
+    if (rc != PBRT_OK) return rc;
+    if (n == 0) return PBRT_OK;
+    DMotion mo;
+    std::memset(&mo, 0, sizeof mo);
+    motion_create(at->start, at->start_inv, at->start_time, at->end, at->end_inv, at->end_time, mo);
+    DevBuf<float> dt, dm, dmi;
+    CK(dt.alloc(n)); CK(dm.alloc(16 * (size_t)n)); CK(dmi.alloc(16 * (size_t)n));
+    CK(cudaMemcpy(dt.p, times, (size_t)n * 4, cudaMemcpyHostToDevice));
+    k_kat_motion<<<(n + 255) / 256, 256>>>(mo, dt.p, n, dm.p, dmi.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    g_launches++;
+    CK(cudaMemcpy(m_out, dm.p, (size_t)n * 64, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(m_inv_out, dmi.p, (size_t)n * 64, cudaMemcpyDeviceToHost));
     return PBRT_OK;
 }
 

@@ -303,6 +303,11 @@ struct PbrtHost {
     std::vector<LightDecl> light_decls;
     // camera / film / sampler / integrator state
     M4 camera_to_world = m4_identity();
+    float transform_times[2] = {0.0f, 1.0f};  // TransformTimes (api.rs:2525-2529)
+    bool have_camera_end = false;             // the camera's end keyframe (ActiveTransform EndTime at the Camera directive)
+    M4 camera_to_world_end = m4_identity();
+    PbrtAnimatedTransform camera_motion;      // built by pbrt_host_world_end
+    PbrtMotionDesc motion;
     int xres = 1280, yres = 720;
     float crop[4] = {0, 1, 0, 1};
     std::string filter = "box";
@@ -556,6 +561,21 @@ int pbrt_host_look_at(PbrtHost* h, const float eye[3], const float look[3], cons
     c2w.m[0][1] = new_up.x; c2w.m[1][1] = new_up.y; c2w.m[2][1] = new_up.z; c2w.m[3][1] = 0.0f;
     c2w.m[0][2] = dir.x; c2w.m[1][2] = dir.y; c2w.m[2][2] = dir.z; c2w.m[3][2] = 0.0f;
     h->camera_to_world = c2w;
+    return 0;
+}
+
+int pbrt_host_transform_times(PbrtHost* h, float start, float end) {  // api.rs:2525-2529
+    if (!h) return hfail(PBRT_E_INVALID, "null argument");
+    h->transform_times[0] = start; h->transform_times[1] = end;
+    h->built = false;
+    return 0;
+}
+
+int pbrt_host_camera_motion(PbrtHost* h, const float* camera_to_world_end) {
+    if (!h) return hfail(PBRT_E_INVALID, "null argument");
+    h->have_camera_end = camera_to_world_end != nullptr;
+    if (camera_to_world_end) std::memcpy(h->camera_to_world_end.m, camera_to_world_end, 64);
+    h->built = false;
     return 0;
 }
 
@@ -885,6 +905,18 @@ int pbrt_host_world_end(PbrtHost* h, uint32_t max_prims_in_node, int n_threads) 
     d.lights = h->lights.data(); d.n_lights = (uint32_t)h->lights.size();
     d.instances = h->instances.empty() ? nullptr : h->instances.data(); d.n_instances = (uint32_t)h->instances.size();
     d.camera = h->cam;
+    // make_camera (api.rs:497-502): AnimatedTransform::new(camera_to_world.t[0], start time, camera_to_world.t[1], end time)
+    std::memset(&h->motion, 0, sizeof h->motion);
+    if (h->have_camera_end) {
+        PbrtAnimatedTransform& a = h->camera_motion;
+        M4 start;  // the camera's camera_to_world as pbrt_host_camera_perspective captured it: m and m_inv of one matrix
+        std::memcpy(start.m, h->cam.camera_to_world, 64);
+        const M4 inv0 = m4_inverse(start), inv1 = m4_inverse(h->camera_to_world_end);
+        std::memcpy(a.start, start.m, 64); std::memcpy(a.start_inv, inv0.m, 64);
+        std::memcpy(a.end, h->camera_to_world_end.m, 64); std::memcpy(a.end_inv, inv1.m, 64);
+        a.start_time = h->transform_times[0]; a.end_time = h->transform_times[1];
+        h->motion.camera = &a;
+    }
     if (!h->nodes.empty()) for (int k = 0; k < 3; ++k) { d.world_bound[k] = h->nodes[0].pmin[k]; d.world_bound[3 + k] = h->nodes[0].pmax[k]; }  // scene.rs:28
     // ---- Film::new / get_sample_bounds (film.rs:176-223,266-289) ----
     PbrtRenderParams& rp = h->rp;
@@ -930,12 +962,13 @@ int pbrt_host_world_end(PbrtHost* h, uint32_t max_prims_in_node, int n_threads) 
 }
 
 const PbrtSceneDesc* pbrt_host_scene_desc(const PbrtHost* h) { return (h && h->built) ? &h->desc : nullptr; }
+const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h) { return (h && h->built && h->motion.camera) ? &h->motion : nullptr; }
 const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h) { return (h && h->built) ? &h->rp : nullptr; }
 
 int pbrt_host_render(PbrtHost* h, int device, const int32_t* pixel_rect, PbrtStats* stats) {
     if (!h || !h->built) return hfail(PBRT_E_INVALID, "pbrt_host_world_end has not run");
     PbrtScene* sc = nullptr;
-    int rc = pbrt_gpu_scene_create(&h->desc, device, &sc);
+    int rc = pbrt_gpu_scene_create_motion(&h->desc, pbrt_host_motion_desc(h), device, &sc);
     if (rc != PBRT_OK) return hfail(rc, pbrt_gpu_last_error());
     const int32_t* rect = pixel_rect ? pixel_rect : h->rp.sample_bounds;
     rc = pbrt_gpu_render(sc, &h->rp, rect, h->film.data(), stats);

@@ -179,6 +179,17 @@ class HostScene:
         self.log.append(("look_at", dict(eye=e.copy(), look=l.copy(), up=u.copy())))
         self._ck(self.L.pbrt_host_look_at(self.h, _fptr(e), _fptr(l), _fptr(u)))
 
+    def transform_times(self, start=0.0, end=1.0):
+        """TransformTimes: the times of the start and end keyframes of every animated transform."""
+        self.log.append(("transform_times", dict(start=float(start), end=float(end))))
+        self._ck(self.L.pbrt_host_transform_times(self.h, start, end))
+
+    def camera_motion(self, camera_to_world_end):
+        """The camera's end keyframe (camera-to-world at the end time, 4x4); the start keyframe is look_at's.  None = static."""
+        m = _f32(camera_to_world_end, (4, 4)) if camera_to_world_end is not None else None
+        self.log.append(("camera_motion", dict(m=None if m is None else m.copy())))
+        self._ck(self.L.pbrt_host_camera_motion(self.h, _fptr(m.reshape(-1)) if m is not None else None))
+
     def film(self, xres, yres, crop=None, filter="box", xwidth=0.5, ywidth=0.5, alpha=2.0, max_sample_luminance=float("inf")):
         c = _f32(crop)
         self.log.append(("film", dict(xres=int(xres), yres=int(yres), crop=None if c is None else c.copy(), filter=filter, xwidth=float(xwidth), ywidth=float(ywidth), alpha=float(alpha),
@@ -263,6 +274,12 @@ class HostScene:
     def params(self):
         return self.L.pbrt_host_render_params(self.h)
 
+    @property
+    def motion(self):
+        """The PbrtMotionDesc of the built scene, or None when nothing in it is animated."""
+        p = self.L.pbrt_host_motion_desc(self.h)
+        return p if p else None
+
     def film_shape(self):
         cb = self.params.contents.cropped_pixel_bounds
         return (cb[3] - cb[1], cb[2] - cb[0])
@@ -297,12 +314,16 @@ class HostScene:
 
 
 class GpuScene:
-    """A scene resident on one GPU: pbrt_gpu_scene_create / render / intersect (include/pbrt_gpu.h)."""
+    """A scene resident on one GPU: pbrt_gpu_scene_create / render / intersect (include/pbrt_gpu.h).  `motion`: a PbrtMotionDesc (or a
+    pointer to one, e.g. HostScene.motion) for pbrt_gpu_scene_create_motion."""
 
-    def __init__(self, desc, device=0, lib=None):
+    def __init__(self, desc, device=0, lib=None, motion=None):
         self.L = lib if lib is not None else _abi.load()  # `lib`: tests may pass another build of the same C ABI
         self.handle = C.c_void_p()
-        rc = self.L.pbrt_gpu_scene_create(desc, device, C.byref(self.handle))
+        if motion is not None:
+            rc = self.L.pbrt_gpu_scene_create_motion(desc, motion if isinstance(motion, C._Pointer) else C.byref(motion), device, C.byref(self.handle))
+        else:
+            rc = self.L.pbrt_gpu_scene_create(desc, device, C.byref(self.handle))
         if rc != 0:
             raise PbrtError(rc, self.L.pbrt_gpu_last_error().decode())
 

@@ -167,7 +167,7 @@ def write(h, path, ply_threshold=2000):
     mesh_i = 0
     in_object = False
     objects = 0
-    film = sampler = integrator = camera = look = None
+    film = sampler = integrator = camera = look = camera_end = times = None
     for name, a in h.log:
         if name == "material":
             materials.append(a)
@@ -256,6 +256,10 @@ def write(h, path, ply_threshold=2000):
             world.append(s)
         elif name == "look_at":
             look = "LookAt %s  %s  %s" % (_nums(a["eye"]), _nums(a["look"]), _nums(a["up"]))
+        elif name == "transform_times":
+            times = a
+        elif name == "camera_motion":
+            camera_end = a["m"]
         elif name == "film":
             film = a
         elif name == "camera":
@@ -266,10 +270,18 @@ def write(h, path, ply_threshold=2000):
             integrator = a
         elif name == "instancing" and a["mode"] != "reference":
             notes.append('instancing "fixed" (pbrt-v3 behaviour) is a library switch; rs_pbrt itself renders the "reference" behaviour (quirk Q7)')
-    if look:
+    if times:
+        pre.append("TransformTimes %r %r" % (times["start"], times["end"]))
+    if camera_end is not None:  # the CTM at the Camera directive is world_to_camera: the end keyframe goes in as its inverse
+        notes.append("camera end keyframe: written as the f32 inverse of camera_to_world, which rs_pbrt inverts again")
+        w2c_end = np.linalg.inv(np.asarray(camera_end, np.float64)).astype(np.float32)
+        pre += ["ActiveTransform StartTime"] + ([look] if look else []) + ["ActiveTransform EndTime", "Transform [%s]" % _nums(w2c_end.T), "ActiveTransform All"]
+    elif look:
         pre.append(look)
     c = camera or {}
     s = 'Camera "perspective" "float fov" [%r]' % c.get("fov", 90.0)
+    if (c.get("shutteropen", 0.0), c.get("shutterclose", 1.0)) != (0.0, 1.0):
+        s += ' "float shutteropen" [%r] "float shutterclose" [%r]' % (c["shutteropen"], c["shutterclose"])
     if c.get("lensradius", 0.0) > 0.0:
         s += ' "float lensradius" [%r] "float focaldistance" [%r]' % (c["lensradius"], c["focaldistance"])
     if c.get("screenwindow") is not None:

@@ -36,7 +36,7 @@ def _box(corners_bottom, height_pts):
 
 def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filter="box", xwidth=0.5, ywidth=0.5, lensradius=0.0,
                 focaldistance=1e6, n_threads=8, crop=None, materials="matte", lights="area", sampler="sobol", samplepixelcenter=False, integrator="path", textures=None, lightsamples=1,
-                alpha=None, quantize_textures=False):
+                alpha=None, quantize_textures=False, camera_end=None, shutter=(0.0, 1.0), transform_times=(0.0, 1.0)):
     """Canonical Cornell box: 5 walls, short and tall block, ceiling light quad (2 triangles => 2 area lights, so
     the spatial light distribution is active).  32 triangles.  `materials="mixed"` swaps the blocks to glass /
     metal and the floor to plastic for BxDF coverage ("translucent", "mix": TranslucentMaterial / MixMaterial on blocks, floor and back wall).  `lights`: "area" (the ceiling quad only), "delta" (plus a point, a spot
@@ -176,12 +176,45 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
     if lights in ("delta", "distant"):
         h.light_distant([0.3, 1.0, -1.5], [0.0, 0.0, 0.0], [1.5, 1.4, 1.1])  # shines in through the open front
     h.look_at([278, 273, -800], [278, 273, 0], [0, 1, 0])
+    _camera_motion(h, camera_end, transform_times)
     h.film(xres, yres, crop=crop, filter=filter, xwidth=xwidth, ywidth=ywidth)
-    h.camera(fov=39.3077, lensradius=lensradius, focaldistance=focaldistance)
+    h.camera(fov=39.3077, lensradius=lensradius, focaldistance=focaldistance, shutteropen=shutter[0], shutterclose=shutter[1])
     h.sampler(spp, name=sampler, samplepixelcenter=samplepixelcenter)
     _set_integrator(h, integrator, maxdepth, strategy)
     h.world_end(n_threads=n_threads)
     return h
+
+
+def look_at_matrix(eye, look, up):
+    """camera_to_world of `LookAt eye look up` (Transform::look_at, transform.rs:414-451), f32, row-major 4x4."""
+    eye, look, up = (np.asarray(v, np.float32) for v in (eye, look, up))
+    d = look - eye
+    d = d / np.sqrt(np.sum(d * d))
+    u = up / np.sqrt(np.sum(up * up))
+    left = np.cross(u, d)
+    left = left / np.sqrt(np.sum(left * left))
+    m = np.eye(4, dtype=np.float32)
+    m[:3, 0], m[:3, 1], m[:3, 2], m[:3, 3] = left, np.cross(d, left), d, eye
+    return m
+
+
+def _camera_motion(h, camera_end, transform_times):
+    """An animated camera: `camera_end` is camera_to_world at the end time (None: static camera, nothing is declared)."""
+    if camera_end is None:
+        return
+    h.transform_times(*transform_times)
+    h.camera_motion(camera_end)
+
+
+def motion_cornell(xres=64, yres=64, spp=16, dolly=150.0, pan=0.0, shutter=(0.0, 1.0), transform_times=(0.0, 1.0), **kw):
+    """The Cornell box seen by an animated camera: over TransformTimes it moves `dolly` units towards the box and turns its view by
+    `pan` degrees about the vertical axis (a rotation keyframe: slerp); `shutter` = (shutteropen, shutterclose).  Other keyword
+    arguments go to cornell_box (materials, lights, textures, lensradius, sampler, integrator, ...)."""
+    a = np.radians(pan)
+    eye = [278.0, 273.0, -800.0 + dolly]
+    look = [eye[0] + 800.0 * np.sin(a), 273.0, eye[2] + 800.0 * np.cos(a)]
+    return cornell_box(xres=xres, yres=yres, spp=spp, camera_end=look_at_matrix(eye, look, [0, 1, 0]), shutter=shutter,
+                       transform_times=transform_times, **kw)
 
 
 def _set_integrator(h, integrator, maxdepth, strategy):
@@ -328,10 +361,12 @@ def _fbm(u, v, rng, octaves=6):
     return out
 
 
-def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, with_normals=True, n_threads=8, crop=None, integrator="path"):
+def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, with_normals=True, n_threads=8, crop=None, integrator="path",
+           dolly=0.0):
     """Ganesha stand-in (config C3): an fBm-displaced, vertically stretched UV sphere of 2*n_side^2 triangles
     (n_side=1468 -> 4.31 M) with per-vertex normals, on a ground quad, lit by 3 rectangular area lights
-    (6 light triangles); matte statue + plastic ground."""
+    (6 light triangles); matte statue + plastic ground.  `dolly` != 0: the camera moves that far towards the statue over the
+    shutter interval (motion blur)."""
     rng = np.random.default_rng(seed)
     h = HostScene()
     body = h.material(_abi.MAT_MATTE, [0.62, 0.47, 0.33, 0.0])
@@ -374,6 +409,9 @@ def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, wi
         h.trianglemesh(*_quad([cx - sx, cy, cz - sz], [cx + sx, cy, cz - sz], [cx + sx, cy, cz + sz], [cx - sx, cy, cz + sz]), material=lm,
                        emit=[float(t) for t in L])
     h.look_at([0.0, 3.2, -7.5], [0.0, 2.0, 0.0], [0, 1, 0])
+    if dolly:
+        eye = np.array([0.0, 3.2, -7.5]) + dolly * np.array([0.0, -1.2, 7.5]) / np.linalg.norm([0.0, -1.2, 7.5])
+        _camera_motion(h, look_at_matrix(eye, [0.0, 2.0, 0.0], [0, 1, 0]), (0.0, 1.0))
     h.film(xres, yres, crop=crop)
     h.camera(fov=38.0)
     h.sampler(spp)
