@@ -1836,21 +1836,20 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 if (!folded) shade_plan.insert(shade_plan.begin(), ShadeLaunch{shade_spec ? (int)lam : 0, 1u, 2u});
             }
         }
-        // Two batches in flight on two streams: k_trace is issue bound, k_shade latency bound, so letting one batch
+        // Two batches in flight on two streams: k_trace and k_shade leave the SMs idle in different ways, so letting one batch
         // trace while the other shades fills the SMs better than either alone.  Disabled for the roofline timing pass
         // (PBRT_RENDER_SINGLE_STREAM: kernel durations must not be inflated by a co-resident kernel), when the queue
         // has to be polled from the host (null materials), and when there is only one batch.
         static const bool dual_env = !(getenv("PB_SINGLE_STREAM") && atoi(getenv("PB_SINGLE_STREAM")));
-        // ... and, since the batches grew to 2^24 camera samples, when an iteration is only one or two k_shade launches: a frame of few
-        // large kernels was expected to fill the GPU by itself, a second batch only competing for cache and registers, while the
-        // conference scene's eight small per-class launches leave room for it.  On an H100 the statue (two launches per iteration) is
-        // about 6 % faster with two batches (DESIGN.md section 7); Cornell and the landscape are not yet measured there, so the rule
-        // stands until they are.  PB_STREAMS >= 2 forces two batches in flight.
+        // ... and when an iteration is a single k_shade launch.  On an H100 at 400 W (DESIGN.md section 7) the statue, two launches per
+        // iteration, renders at 1 629-1 637 Mrays/s with two batches in flight against 1 574-1 585 with one; Cornell, one Lambert launch,
+        // cannot be told apart (2 873-2 953 against 2 902-2 969), so it keeps one stream.  PB_STREAMS = 1 keeps one batch in flight,
+        // PB_STREAMS >= 2 forces two.
         // A textured frame is bound by k_texture's per-hit records (written once, read back by k_shade): a second batch in flight doubles that
         // working set and loses.
         const bool streams_forced = getenv("PB_STREAMS") && atoi(getenv("PB_STREAMS")) >= 2;
         const bool dual = dual_env && !(p->flags & PBRT_RENDER_SINGLE_STREAM) && !null_paths && n_batches > 1 &&
-                          !(getenv("PB_STREAMS") && atoi(getenv("PB_STREAMS")) <= 1) && ((shade_plan.size() >= 3 && sc->d.n_textures == 0) || streams_forced);
+                          !(getenv("PB_STREAMS") && atoi(getenv("PB_STREAMS")) <= 1) && ((shade_plan.size() >= 2 && sc->d.n_textures == 0) || streams_forced);
         static const int streams_env = getenv("PB_STREAMS") ? std::min(4, std::max(1, atoi(getenv("PB_STREAMS")))) : 2;
         const int n_ctx = dual ? (int)std::min<uint64_t>((uint64_t)streams_env, n_batches) : 1;
 
