@@ -22,7 +22,8 @@
  * 3 = image textures (PbrtTexture, PbrtMaterial.tex / bump, PbrtSceneDesc.textures), PbrtLight.n_samples, the directlighting and
  * whitted integrators (PbrtRenderParams.direct_strategy); 4 = PbrtStats.shade_slots / shaded_vertices, tile-interleaved rendering
  * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi); within 4, the animated camera
- * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed).  Structs only ever grow at their end
+ * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed); within 4, goniometric and projection lights
+ * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word).  Structs only ever grow at their end
  * within a version step, and a zero-initialised new field means "as before".
  */
 #ifndef PBRT_GPU_H
@@ -208,9 +209,24 @@ typedef enum PbrtInstancing { PBRT_INSTANCING_REFERENCE = 0, PBRT_INSTANCING_FIX
  *                 restates InfiniteAreaLight::new: a map whose resolution is not a power of two is resampled to the next one
  *                 (MipMap::new's 4-tap Lanczos zoom, mipmap.rs:60-150), then the MIP pyramid (power()), the 2w x 2h
  *                 Distribution2D (sampling.rs:150-198) and the world radius are derived.
+ *   GONIOMETRIC   GonioPhotometricLight (src/lights/goniometric.rs): L = I * scale, p = p_light, w2l = upper 3x3 of world_to_light,
+ *                 env_res / env_texels = the map exactly as new_hdr hands it to MipMap::new (RGB f32, row 0 = the file's first row: the
+ *                 constructor does not flip rows).  env_texels == NULL means no "mapname": scale(w) is exactly 1.  The radiance toward
+ *                 a point is L * lookup(phi / 2pi, theta / pi) / d^2 of the light-space direction normalize(w2l * w) with y and z
+ *                 swapped (goniometric.rs:233-265).
+ *   PROJECTION    ProjectionLight (src/lights/projection.rs): L, p, w2l and the map as for GONIOMETRIC, fov = "fov" (default 45).
+ *                 The library restates the constructor (screen window from the map's aspect, Transform::perspective(fov, 1e-3,
+ *                 1e30), cos_total_width) and projection(w) (:339-360).  env_texels is required (NULL is PBRT_E_INVALID): a projection
+ *                 light without "mapname" is black in the reference (I = 0, at the origin), and the caller hands it over as a
+ *                 POINT light with L = 0 and p = 0, which gives the same samples, ray counts and power.
+ *   Both: a map larger than 16384 texels on a side is PBRT_E_UNSUPPORTED; a zero resolution with texels, or a p / w2l / fov that is
+ *   not finite (fov outside (0, 180) for PROJECTION) is PBRT_E_INVALID.  Not allowed inside object instances (neither is the reference).
  * Delta lights take the `is_delta_light` branch of estimate_direct (integrator.rs:470-480: no MIS, no BSDF sample). Rays that
  * leave the scene collect Le of every infinite light (path.rs:267-275, integrator.rs:560-562). */
-typedef enum PbrtLightKind { PBRT_LIGHT_DIFFUSE_AREA = 0, PBRT_LIGHT_POINT = 1, PBRT_LIGHT_SPOT = 2, PBRT_LIGHT_DISTANT = 3, PBRT_LIGHT_INFINITE = 4 } PbrtLightKind;
+typedef enum PbrtLightKind {
+    PBRT_LIGHT_DIFFUSE_AREA = 0, PBRT_LIGHT_POINT = 1, PBRT_LIGHT_SPOT = 2, PBRT_LIGHT_DISTANT = 3, PBRT_LIGHT_INFINITE = 4,
+    PBRT_LIGHT_GONIOMETRIC = 5, PBRT_LIGHT_PROJECTION = 6 /* ABI v4 */
+} PbrtLightKind;
 #define PBRT_MAX_INFINITE_LIGHTS 4
 typedef struct PbrtLight {
     uint32_t kind;
@@ -219,13 +235,13 @@ typedef struct PbrtLight {
     uint32_t two_sided;
     float area;        /* area: DiffuseAreaLight.area == Triangle::area() at creation */
     float p[3];        /* point/spot: p_light; distant: w_light */
-    float w2l[9];      /* spot, infinite: world_to_light rotation, row-major */
+    float w2l[9];      /* spot, infinite, goniometric, projection: upper 3x3 of world_to_light, row-major */
     float cos_total_width, cos_falloff_start; /* spot */
     float l2w[9];      /* infinite: light_to_world rotation, row-major */
-    uint32_t env_res[2];      /* infinite: map resolution {width, height} */
-    const float* env_texels;  /* infinite: env_res[0] * env_res[1] RGB texels */
+    uint32_t env_res[2];      /* infinite, goniometric, projection: map resolution {width, height} */
+    const float* env_texels;  /* infinite, goniometric, projection: env_res[0] * env_res[1] RGB texels */
     uint32_t n_samples;       /* "nsamples"/"samples" of the light (Light::get_n_samples; 0 reads as 1): DirectLightingIntegrator "all" */
-    uint32_t pad;
+    float fov;                /* projection: "fov" in degrees (was a zero pad word: the layout is unchanged) */
 } PbrtLight;
 
 /* PerspectiveCamera (src/cameras/perspective.rs:23-43); row-major 4x4, m[r][c] = a[4*r+c].

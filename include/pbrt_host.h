@@ -80,6 +80,13 @@ int pbrt_host_add_light_distant(PbrtHost* h, const float from[3], const float to
 /* LightSource "infinite": texels = NULL for a constant light (InfiniteAreaLight::default, infinite.rs:250-300), else a
  * width x height RGB lat-long map (any resolution) that is multiplied by L*scale as the reference does on load.
  * light_to_world / world_to_light: row-major 3x3 rotations of the CTM and its inverse, both NULL for identity. */
+/* LightSource "goniometric" / "projection" under the current transform: light_to_world / world_to_light are the CTM and its inverse
+ * (row-major 4x4), texels an RGB map of width x height with row 0 first as the .hdr file stores it (NULL: no "mapname"; required for
+ * a projection light), fov in degrees (the reference's default is 45). */
+int pbrt_host_add_light_goniometric(PbrtHost* h, const float I[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
+                                    const float light_to_world[16], const float world_to_light[16]);
+int pbrt_host_add_light_projection(PbrtHost* h, const float I[3], const float scale[3], const float* texels, uint32_t width, uint32_t height, float fov,
+                                   const float light_to_world[16], const float world_to_light[16]);
 int pbrt_host_add_light_infinite(PbrtHost* h, const float L[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
                                  const float* light_to_world, const float* world_to_light);
 int pbrt_host_look_at(PbrtHost* h, const float eye[3], const float look[3], const float up[3]);

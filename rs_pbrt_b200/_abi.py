@@ -13,7 +13,7 @@ LIB_PATH = Path(os.environ.get("RS_PBRT_B200_LIB") or Path(__file__).resolve().p
 
 PBRT_OK, PBRT_E_INVALID, PBRT_E_UNSUPPORTED, PBRT_E_CUDA, PBRT_E_NO_DEVICE = 0, -1, -2, -3, -4
 PBRT_NO_MATERIAL = 0xFFFFFFFF
-LIGHT_DIFFUSE_AREA, LIGHT_POINT, LIGHT_SPOT, LIGHT_DISTANT, LIGHT_INFINITE = range(5)
+LIGHT_DIFFUSE_AREA, LIGHT_POINT, LIGHT_SPOT, LIGHT_DISTANT, LIGHT_INFINITE, LIGHT_GONIOMETRIC, LIGHT_PROJECTION = range(7)
 MAT_MATTE, MAT_PLASTIC, MAT_METAL, MAT_MIRROR, MAT_GLASS, MAT_UBER, MAT_SUBSTRATE, MAT_TRANSLUCENT, MAT_MIX = range(9)
 LIGHTS_UNIFORM, LIGHTS_POWER, LIGHTS_SPATIAL = 0, 1, 2
 SAMPLER_SOBOL, SAMPLER_HALTON = 0, 1
@@ -55,7 +55,7 @@ class PbrtMaterial(C.Structure):
 class PbrtLight(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("L", C.c_float * 3), ("tri", C.c_uint32), ("two_sided", C.c_uint32), ("area", C.c_float),
                 ("p", C.c_float * 3), ("w2l", C.c_float * 9), ("cos_total_width", C.c_float), ("cos_falloff_start", C.c_float),
-                ("l2w", C.c_float * 9), ("env_res", C.c_uint32 * 2), ("env_texels", C.POINTER(C.c_float)), ("n_samples", C.c_uint32), ("pad", C.c_uint32)]
+                ("l2w", C.c_float * 9), ("env_res", C.c_uint32 * 2), ("env_texels", C.POINTER(C.c_float)), ("n_samples", C.c_uint32), ("fov", C.c_float)]
 
 
 class PbrtInstance(C.Structure):
@@ -107,7 +107,7 @@ GPU_SYMBOLS = ["pbrt_gpu_scene_create", "pbrt_gpu_scene_destroy", "pbrt_gpu_scen
                "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2",
                "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate"]
 HOST_SYMBOLS = ["pbrt_host_new", "pbrt_host_free", "pbrt_host_last_error", "pbrt_host_add_material", "pbrt_host_add_material_mix", "pbrt_host_add_trianglemesh",
-                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
+                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
                 "pbrt_host_integrator_path", "pbrt_host_world_end", "pbrt_host_scene_desc", "pbrt_host_render_params", "pbrt_host_render",
                 "pbrt_host_film_rgbw", "pbrt_host_film_clear", "pbrt_host_film_add_rgbw", "pbrt_host_film_rgb", "pbrt_host_write_image",
                 "pbrt_host_bvh_build"]
@@ -166,6 +166,8 @@ def bind(L):
     L.pbrt_host_add_light_spot.argtypes = [vp, fp, fp, fp, fp, C.c_float, C.c_float]
     L.pbrt_host_add_light_distant.argtypes = [vp, fp, fp, fp, fp]
     L.pbrt_host_add_light_infinite.argtypes = [vp, fp, fp, fp, C.c_uint32, C.c_uint32, fp, fp]
+    L.pbrt_host_add_light_goniometric.argtypes = [vp, fp, fp, fp, C.c_uint32, C.c_uint32, fp, fp]
+    L.pbrt_host_add_light_projection.argtypes = [vp, fp, fp, fp, C.c_uint32, C.c_uint32, C.c_float, fp, fp]
     L.pbrt_host_look_at.argtypes = [vp, fp, fp, fp]
     L.pbrt_host_transform_times.argtypes = [vp, C.c_float, C.c_float]
     L.pbrt_host_camera_motion.argtypes = [vp, fp]

@@ -386,6 +386,7 @@ __global__ void __launch_bounds__(128) k_direct_step(DScene sc, DRender rp, DPat
 }
 
 // estimate_direct (integrator.rs:406-570) for light sample q of the node shaded in this iteration, up to its two rays
+template <int LIGHTS>
 __global__ void __launch_bounds__(128) k_direct_nee(DScene sc, DRender rp, DPaths ps, DDirect dd, BatchInfo bi, const uint32_t* __restrict__ nib,
                                                     const uint64_t* __restrict__ vdc, const uint64_t* __restrict__ vdci, float4* __restrict__ rays,
                                                     uint32_t* __restrict__ d_nrays, DCounters* cnt, uint32_t* __restrict__ d_error,
@@ -474,7 +475,7 @@ __global__ void __launch_bounds__(128) k_direct_nee(DScene sc, DRender rp, DPath
                 V3 wi = mk3(0.0f, 0.0f, 0.0f);
                 float light_pdf = 0.0f, scattering_pdf = 0.0f;
                 LightSample ls;
-                const Sp li = light_sample_li<false>(sc, light, is.p, u_light, wi, light_pdf, ls);
+                const Sp li = light_sample_li<LIGHTS>(sc, light, is.p, u_light, wi, light_pdf, ls);
                 if (dd.whitted) {  // whitted.rs:84-96
                     if (!(is_black(li) || light_pdf == 0.0f)) {
                         const Sp f = bsdf_f(B, wo, wi, BSDF_ALL);
@@ -498,7 +499,7 @@ __global__ void __launch_bounds__(128) k_direct_nee(DScene sc, DRender rp, DPath
                             const V3 origin = offset_ray_origin(is.p, is.p_error, is.n, ls.p - is.p);
                             const V3 target = offset_ray_origin(ls.p, ls.p_error, ls.n, origin - ls.p);
                             const V3 sd = target - origin;
-                            if (light_is_delta(light)) a = f * li / light_pdf;
+                            if (light_is_delta<LIGHTS>(light)) a = f * li / light_pdf;
                             else a = f * li * sp1(power_heuristic(light_pdf, scattering_pdf)) / light_pdf;
                             sh0 = make_float4(origin.x, origin.y, origin.z, 1.0f - PB_SHADOW_EPSILON);
                             sh1 = make_float4(sd.x, sd.y, sd.z, __uint_as_float((uint32_t)r | (RAY_SHADOW << 30)));
@@ -506,14 +507,14 @@ __global__ void __launch_bounds__(128) k_direct_nee(DScene sc, DRender rp, DPath
                             flags |= 1u;
                         }
                     }
-                    if (!light_is_delta(light)) {
+                    if (!light_is_delta<LIGHTS>(light)) {
                         int st = 0;
                         Sp f2 = bsdf_sample_f(B, wo, wi, u_scat, scattering_pdf, NONSPEC, st);
                         f2 = f2 * sp1(absdot3(wi, is.ns));
                         if (!is_black(f2) && scattering_pdf > 0.0f) {
                             const V3 mo = offset_ray_origin(is.p, is.p_error, is.n, wi);
                             if (light.kind == 0u) n_light_tests++;
-                            const float lp = light_pdf_li<false>(sc, light, is.p, mo, wi);
+                            const float lp = light_pdf_li<LIGHTS>(sc, light, is.p, mo, wi);
                             if (lp != 0.0f) {
                                 mis_w = power_heuristic(scattering_pdf, lp);
                                 mis0 = make_float4(mo.x, mo.y, mo.z, __int_as_float(0x7f800000));

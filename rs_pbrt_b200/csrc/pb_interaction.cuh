@@ -289,18 +289,48 @@ PB_D float env_pdf_li(const DEnv& e, V3 w) {
     float map_pdf = __ldg(e.cond_func + (size_t)iv * e.nu + iu) / e.marg_int;
     return map_pdf / (2.0f * PB_PI * PB_PI * sin_theta);
 }
-PB_D bool light_is_delta(const DLight& l) { return l.kind - 1u < 3u; }  // point, spot, distant (light.rs:178-190)
+// Light levels of the kernels that sample lights, fixed per scene at creation: 0 = DiffuseAreaLights only (the other kinds are compiled
+// out), 1 = every kind but the image lights, 2 = with GonioPhotometricLight / ProjectionLight (their own instantiations, so the others
+// keep their code).
+template <int LIGHTS>
+PB_D bool light_is_delta(const DLight& l) {  // point, spot, distant, goniometric, projection (light.rs:178-190)
+    return LIGHTS >= 2 ? (l.kind - 1u < 3u || l.kind - 5u < 2u) : l.kind - 1u < 3u;
+}
 // Light::le (light.rs:84-94): zero for everything but an infinite light
 PB_D Sp light_le(const DScene& sc, const DLight& l, V3 ray_d) {
     if (l.kind != 4u) return sp1(0.0f);
     return env_le(sc.envs[l.env], ray_d);
 }
 
-// Light::sample_li: DiffuseAreaLight (diffuse.rs:64-84), PointLight, SpotLight, DistantLight (lights/{point,spot,distant}.rs).
+// GonioPhotometricLight::scale (goniometric.rs:233-248) or ProjectionLight::projection (projection.rs:339-360) of the world direction
+// w: a level-0 bilinear lookup of the map (lookup_pnt_flt(st, 0)), or exactly 1 for a goniometric light without one.
+PB_D Sp image_light_scale(const DLight& l, const DEnv& e, V3 w) {
+    if (l.kind == 5u) {
+        if (e.w == 0) return sp1(1.0f);
+        const V3 wn = norm3(rot3(l.w2l, w));
+        const V3 wp = mk3(wn.x, wn.z, wn.y);  // std::mem::swap(&mut wp.y, &mut wp.z)
+        return env_lookup(e, spherical_phi(wp) * PB_INV_2_PI, spherical_theta(wp) * PB_INV_PI);
+    }
+    const V3 wl = rot3(l.w2l, w);  // not normalised
+    if (wl.z < e.hither) return sp1(0.0f);
+    const float* m = e.proj;  // Transform::transform_point: the homogeneous divide multiplies by 1 / wp
+    float px = m[0] * wl.x + m[1] * wl.y + m[2] * wl.z + m[3];
+    float py = m[4] * wl.x + m[5] * wl.y + m[6] * wl.z + m[7];
+    const float pw = m[12] * wl.x + m[13] * wl.y + m[14] * wl.z + m[15];
+    if (pw != 1.0f) { const float inv = 1.0f / pw; px = inv * px; py = inv * py; }
+    if (!(px >= e.screen[0] && px <= e.screen[2] && py >= e.screen[1] && py <= e.screen[3])) return sp1(0.0f);  // pnt2_inside_bnd2f
+    float sx = px - e.screen[0], sy = py - e.screen[1];  // Bounds2f::offset
+    if (e.screen[2] > e.screen[0]) sx /= e.screen[2] - e.screen[0];
+    if (e.screen[3] > e.screen[1]) sy /= e.screen[3] - e.screen[1];
+    return env_lookup(e, sx, sy);
+}
+
+// Light::sample_li: DiffuseAreaLight (diffuse.rs:64-84), PointLight, SpotLight, DistantLight (lights/{point,spot,distant}.rs),
+// GonioPhotometricLight and ProjectionLight (goniometric.rs:249-265, projection.rs:362-378) at light level 2.
 // For the delta lights the sampled "interaction" is a bare point (n = p_error = 0).
-// AREA_ONLY: the scene holds DiffuseAreaLights only (known at scene creation), the other kinds are compiled out
-template <bool AREA_ONLY>
+template <int LIGHTS>
 PB_D Sp light_sample_li(const DScene& sc, const DLight& l, V3 ref_p, float2 u, V3& wi, float& pdf, LightSample& ls) {
+    constexpr bool AREA_ONLY = LIGHTS == 0;
     if (!AREA_ONLY && l.kind == 4u) {  // InfiniteAreaLight::sample_li
         const DEnv& e = sc.envs[l.env];
         ls.p_error = mk3(0.0f, 0.0f, 0.0f);
@@ -336,6 +366,7 @@ PB_D Sp light_sample_li(const DScene& sc, const DLight& l, V3 ref_p, float2 u, V
         wi = norm3(lp - ref_p);
         ls.p = lp;
         float d2 = len2(lp - ref_p);
+        if (LIGHTS >= 2 && l.kind >= 5u) return I * image_light_scale(l, sc.envs[l.env], -wi) / d2;
         if (l.kind == 1u) return I / d2;
         return I * spot_falloff(l, -wi) / d2;
     }
@@ -345,9 +376,9 @@ PB_D Sp light_sample_li(const DScene& sc, const DLight& l, V3 ref_p, float2 u, V
     return light_L(l, ls.n, -wi);
 }
 // DiffuseAreaLight::pdf_li for the ray (o, wi) spawned from the shaded point ref_p
-template <bool AREA_ONLY>
+template <int LIGHTS>
 PB_D float light_pdf_li(const DScene& sc, const DLight& l, V3 ref_p, V3 ray_o, V3 wi) {
-    if (!AREA_ONLY && l.kind == 4u) return env_pdf_li(sc.envs[l.env], wi);
+    if (LIGHTS != 0 && l.kind == 4u) return env_pdf_li(sc.envs[l.env], wi);
     V3 p0, p1, p2;
     load_tri(sc.tri_verts, l.tri, p0, p1, p2);
     RayPre r = make_ray(ray_o, wi);

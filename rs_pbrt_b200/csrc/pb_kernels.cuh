@@ -541,6 +541,7 @@ __global__ void __launch_bounds__(256) k_sort(DScene sc, DPaths ps, DLightGrid g
 // SpatialLightDistribution::compute_distribution (lightdistrib.rs:169-269), split in two kernels:
 // one thread per (requested voxel, light) accumulates the 128 Halton samples IN ORDER, then one
 // thread per voxel builds the Distribution1D (sampling.rs:24-49).
+template <int LIGHTS>
 __global__ void k_lightgrid_contrib(DScene sc, DLightGrid g, const float* __restrict__ halton /* 128 x 5 */) {
     uint32_t nreq = *g.n_request;
     uint32_t total = nreq * (uint32_t)g.n_lights;
@@ -559,7 +560,7 @@ __global__ void k_lightgrid_contrib(DScene sc, DLightGrid g, const float* __rest
             float pdf = 0.0f;
             V3 wi;
             LightSample ls;
-            Sp li = light_sample_li<false>(sc, light, po, make_float2(__ldg(hs + 3), __ldg(hs + 4)), wi, pdf, ls);
+            Sp li = light_sample_li<LIGHTS>(sc, light, po, make_float2(__ldg(hs + 3), __ldg(hs + 4)), wi, pdf, ls);
             if (pdf > 0.0f) contrib += lum(li) / pdf;
         }
         g.contrib[g.row_of(v) * g.n_lights + j] = contrib;
@@ -830,7 +831,7 @@ __global__ void __launch_bounds__(128) k_texture(DScene sc, DRender rp, DPaths p
 // (104-200 B of stack) and were slower on the statue, Cornell and the conference scene on an H100 SXM (700 W).
 #define PB_SHADE_SPEC_BLOCKS 4
 #endif
-template <bool AREA_ONLY, bool HALTON, bool INST, int SPEC>
+template <int LIGHTS, bool HALTON, bool INST, int SPEC>
 __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_BLOCKS : 4)) k_shade(DScene sc, DRender rp, DPaths ps, DLightGrid grid, const uint32_t* __restrict__ nib,
                                                           uint32_t sobol_cfg, uint32_t n_chunks, const uint32_t* __restrict__ cls_queue,
                                                           uint32_t cls_stride, const uint32_t* __restrict__ cls_count, uint32_t* __restrict__ queue_out,
@@ -978,7 +979,7 @@ __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_B
                                 float light_pdf = 0.0f, scattering_pdf = 0.0f, mis_w = 0.0f;
                                 Sp a = sp1(0.0f);
                                 LightSample ls;
-                                Sp li = light_sample_li<AREA_ONLY>(sc, light, is.p, u_light, wi, light_pdf, ls);
+                                Sp li = light_sample_li<LIGHTS>(sc, light, is.p, u_light, wi, light_pdf, ls);
                                 if (light_pdf > 0.0f && !is_black(li)) {
                                     Sp f = bsdf_f<SPEC>(B, wo_nee, wi, NONSPEC) * sp1(absdot3(wi, is.ns));
                                     scattering_pdf = bsdf_pdf<SPEC>(B, wo_nee, wi, NONSPEC);
@@ -987,7 +988,7 @@ __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_B
                                         V3 origin = offset_ray_origin(is.p, is.p_error, is.n, ls.p - is.p);
                                         V3 target = offset_ray_origin(ls.p, ls.p_error, ls.n, origin - ls.p);
                                         V3 sd = target - origin;
-                                        if (!AREA_ONLY && light_is_delta(light)) a = f * li / light_pdf;  // is_delta_light: no MIS
+                                        if (LIGHTS != 0 && light_is_delta<LIGHTS>(light)) a = f * li / light_pdf;  // is_delta_light: no MIS
                                         else {
                                             float w = power_heuristic(light_pdf, scattering_pdf);
                                             a = f * li * sp1(w) / light_pdf;
@@ -1002,14 +1003,14 @@ __global__ void __launch_bounds__(PB_SHADE_THREADS, (SPEC >= 1 ? PB_SHADE_SPEC_B
                                 // with the light strategy as in the reference, sampled_type = 0 in (quirk Q8)
                                 int st = 0;
                                 Sp f2 = sp1(0.0f);
-                                if (AREA_ONLY || !light_is_delta(light)) {
+                                if (LIGHTS == 0 || !light_is_delta<LIGHTS>(light)) {
                                     f2 = bsdf_sample_f<SPEC>(B, wo_nee, wi, u_scat, scattering_pdf, NONSPEC, st);
                                     f2 = f2 * sp1(absdot3(wi, is.ns));
                                 }
                                 if (!is_black(f2) && scattering_pdf > 0.0f) {
                                     V3 mo = offset_ray_origin(is.p, is.p_error, is.n, wi);  // it.spawn_ray(wi)
-                                    if (AREA_ONLY || light.kind == 0u) n_light_tests++;  // Triangle::intersect inside pdf_li (area lights only)
-                                    float lp = light_pdf_li<AREA_ONLY>(sc, light, is.p, mo, wi);
+                                    if (LIGHTS == 0 || light.kind == 0u) n_light_tests++;  // Triangle::intersect inside pdf_li (area lights only)
+                                    float lp = light_pdf_li<LIGHTS>(sc, light, is.p, mo, wi);
                                     if (lp != 0.0f) {
                                         mis_w = power_heuristic(scattering_pdf, lp);
                                         mis0 = make_float4(mo.x, mo.y, mo.z, inf);

@@ -54,17 +54,28 @@ struct DLight {           // DiffuseAreaLight over one triangle (lights/diffuse.
 };
 // InfiniteAreaLight (lights/infinite.rs): MIP level 0 of the radiance map (every lookup the path makes has width 0 and lands on
 // MipMap::triangle(0, st), mipmap.rs:233-240) and the 2w x 2h Distribution2D (sampling.rs:150-198), stored densely.
+// A GonioPhotometricLight / ProjectionLight (lights/goniometric.rs, projection.rs) has the same kind of record: MIP level 0 of its
+// map (w == 0: no map, scale 1) and, for a projection light, the constants of ProjectionLight::new in place of the distribution.
 struct DEnv {
     const float4* texels;  // w*h, row-major, {r,g,b,_}
     int w, h;              // powers of two
     int nu, nv;            // distribution resolution (2w, 2h)
-    const float* cond_func;  // [nv][nu]
-    const float* cond_cdf;   // [nv][nu+1]
-    const float* cond_int;   // [nv] func_int of each row
-    const float* marg_func;  // [nv]
-    const float* marg_cdf;   // [nv+1]
-    float marg_int;
-    float l2w[9], w2l[9];
+    union {
+        struct {
+            const float* cond_func;  // [nv][nu]
+            const float* cond_cdf;   // [nv][nu+1]
+            const float* cond_int;   // [nv] func_int of each row
+            const float* marg_func;  // [nv]
+            const float* marg_cdf;   // [nv+1]
+            float marg_int;
+            float l2w[9], w2l[9];
+        };
+        struct {
+            float proj[16];     // light_projection.m, row-major (Transform::perspective(fov, hither, yon))
+            float screen[4];    // screen_bounds {pmin.x, pmin.y, pmax.x, pmax.y}
+            float hither;
+        };
+    };
 };
 
 // ImageTexture<Spectrum> (imagemap.rs:17-150): the MIP pyramid of MipMap::new, all levels in one float4 array ({r,g,b,_}, row-major,

@@ -332,6 +332,31 @@ static void build_env(const float* rgb_in, int w, int h, HostEnv& e) {
     }
     make_distribution(e.marg_func, e.marg_cdf, e.marg_int);
 }
+// ProjectionLight::new_hdr (projection.rs:85-225) for a map of aspect = width / height: the screen window, hither, light_projection =
+// Transform::perspective(fov, hither, yon) (transform.rs:461-488) and cos_total_width, the corner of the window through screen_to_light =
+// Transform::inverse(light_projection), which is light_projection.m_inv (transform.rs:285-290).
+static void projection_constants(float aspect, float fov, float* proj, float* screen, float& hither, float& cos_total_width) {
+    if (aspect > 1.0f) { screen[0] = -aspect; screen[1] = -1.0f; screen[2] = aspect; screen[3] = 1.0f; }
+    else { screen[0] = -1.0f; screen[1] = -1.0f / aspect; screen[2] = 1.0f; screen[3] = 1.0f / aspect; }
+    hither = 1e-3f;
+    const float n = hither, f = 1e30f;
+    const float persp[16] = {1.0f, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f, 0.0f, 0.0f, 0.0f, 0.0f, f / (f - n), -f * n / (f - n), 0.0f, 0.0f, 1.0f, 0.0f};
+    float persp_inv[16];
+    mx_inverse(persp, persp_inv);
+    const float inv_tan_ang = 1.0f / tanf((PB_PI / 180.0f) * fov / 2.0f);  // radians(fov) / 2
+    const float scale[16] = {inv_tan_ang, 0.0f, 0.0f, 0.0f, 0.0f, inv_tan_ang, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f};
+    const float scale_inv[16] = {1.0f / inv_tan_ang, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f / inv_tan_ang, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f / 1.0f, 0.0f, 0.0f, 0.0f, 0.0f, 1.0f};
+    float m_inv[16];
+    mx_mul(scale, persp, proj);        // (scale * persp).m
+    mx_mul(persp_inv, scale_inv, m_inv);  // (scale * persp).m_inv
+    const float x = screen[2], y = screen[3], z = 0.0f;  // transform_point(p_corner) with m_inv
+    float xp = m_inv[0] * x + m_inv[1] * y + m_inv[2] * z + m_inv[3];
+    float yp = m_inv[4] * x + m_inv[5] * y + m_inv[6] * z + m_inv[7];
+    float zp = m_inv[8] * x + m_inv[9] * y + m_inv[10] * z + m_inv[11];
+    const float wp = m_inv[12] * x + m_inv[13] * y + m_inv[14] * z + m_inv[15];
+    if (wp != 1.0f) { const float inv = 1.0f / wp; xp = inv * xp; yp = inv * yp; zp = inv * zp; }
+    cos_total_width = norm3(mk3(xp, yp, zp)).z;
+}
 // HaltonSampler tables (samplers/halton.rs:18-26, lowdiscrepancy.rs:18-147,2165-2187, rng.rs, sampling.rs:202-212): the first
 // 1000 primes, their prefix sums, and RADICAL_INVERSE_PERMUTATIONS -- each prime's digits shuffled with PCG32's default
 // stream, prime after prime, so the whole table is one deterministic constant of the reference.
@@ -540,7 +565,7 @@ struct PbrtScene {
     bool has_null_material = false;
     bool cam_motion = false;  // the camera is animated: k_raygen<true> interpolates cam_mo at each sample's time
     DMotion cam_mo;
-    bool area_only = true;  // every light is a DiffuseAreaLight: k_shade<true> has the other kinds compiled out
+    int light_level = 0;  // light level of the kernels that sample lights (pb_interaction.cuh): 0 = area lights only, 1 = any but image lights, 2 = with them
     uint32_t class_mask = 0;  // bit c: some material has shading class c (1..8: a single lobe of kind c - 1; 9: Lambert + microfacet reflection; 10..15: everything else)
     size_t upload_bytes = 0;
     DevBuf<DCounters> counters;
@@ -803,7 +828,7 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     uint32_t n_inf = 0, inf_idx[PBRT_MAX_INFINITE_LIGHTS] = {0, 0, 0, 0};
     for (uint32_t i = 0; i < desc->n_lights; ++i) {
         const PbrtLight& l = desc->lights[i];
-        if (l.kind > PBRT_LIGHT_INFINITE) return fail(PBRT_E_UNSUPPORTED, "light kind outside the GPU path");
+        if (l.kind > PBRT_LIGHT_PROJECTION) return fail(PBRT_E_UNSUPPORTED, "light kind outside the GPU path");
         if (l.kind == PBRT_LIGHT_DIFFUSE_AREA && l.tri >= desc->n_tris) return fail(PBRT_E_INVALID, "light triangle out of range");
         std::memset(&lights[i], 0, sizeof(DLight));
         lights[i].kind = l.kind;
@@ -822,6 +847,17 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
             if (w > 16384 || h > 16384) return fail(PBRT_E_UNSUPPORTED, "environment map larger than 16384 texels on a side");
             if (n_inf == PBRT_MAX_INFINITE_LIGHTS) return fail(PBRT_E_UNSUPPORTED, "too many infinite lights");
             inf_idx[n_inf++] = i;
+        }
+        if (l.kind == PBRT_LIGHT_GONIOMETRIC || l.kind == PBRT_LIGHT_PROJECTION) {
+            const uint32_t w = l.env_res[0], h = l.env_res[1];
+            if (l.env_texels && (w == 0 || h == 0)) return fail(PBRT_E_INVALID, "image light map with a zero resolution");
+            if (!l.env_texels && l.kind == PBRT_LIGHT_PROJECTION) return fail(PBRT_E_INVALID, "projection light without a map (pass it as a black point light)");
+            if (l.env_texels && (w > 16384 || h > 16384)) return fail(PBRT_E_UNSUPPORTED, "image light map larger than 16384 texels on a side");
+            bool finite = true;
+            for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(l.p[k]);
+            for (int k = 0; k < 9; ++k) finite = finite && std::isfinite(l.w2l[k]);
+            if (!finite) return fail(PBRT_E_INVALID, "image light position or world_to_light not finite");
+            if (l.kind == PBRT_LIGHT_PROJECTION && !(l.fov > 0.0f && l.fov < 180.0f)) return fail(PBRT_E_INVALID, "projection light fov outside (0, 180) degrees");
         }
     }
     // The host-side flattening runs on all cores (a 4.3 M-triangle scene is re-uploaded on every end-to-end step).
@@ -1151,7 +1187,7 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     since("tables built");
     sc->has_null_material = has_null;
     sc->h_nib = nib;
-    for (const DLight& l : lights) if (l.kind != PBRT_LIGHT_DIFFUSE_AREA) sc->area_only = false;
+    for (const DLight& l : lights) sc->light_level = std::max(sc->light_level, l.kind == PBRT_LIGHT_DIFFUSE_AREA ? 0 : l.kind < PBRT_LIGHT_GONIOMETRIC ? 1 : 2);
     for (const DMaterial& m : mats) sc->class_mask |= 1u << (m.cls & 0xff);
     sc->h_lights = lights;
 #define UP(buf, vec)                                                                                     \
@@ -1201,6 +1237,34 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
             lights[inf_idx[k]].env = (uint32_t)envs.size();
             envs.push_back(de);
             sc->h_env_power[inf_idx[k]] = he.power_L;
+        }
+        // goniometric and projection lights: MipMap::new (the Lanczos zoom and the pyramid) for level 0 and power()
+        for (uint32_t i = 0; i < desc->n_lights; ++i) {
+            const PbrtLight& l = desc->lights[i];
+            if (l.kind != PBRT_LIGHT_GONIOMETRIC && l.kind != PBRT_LIGHT_PROJECTION) continue;
+            DEnv de;
+            std::memset(&de, 0, sizeof de);
+            Sp lookup_half = sp1(1.0f);  // power(): Spectrum::new(1.0) without a map
+            if (l.env_texels) {
+                std::vector<MipLevel> pyr;
+                build_pyramid(l.env_texels, (int)l.env_res[0], (int)l.env_res[1], PBRT_WRAP_REPEAT, pyr);
+                std::vector<float4> t0((size_t)pyr[0].us * pyr[0].vs);
+                for (size_t q = 0; q < t0.size(); ++q) t0[q] = make_float4(pyr[0].t[q].r, pyr[0].t[q].g, pyr[0].t[q].b, 0.0f);
+                sc->env_bufs.emplace_back(new PbrtScene::EnvBufs());
+                cudaError_t e_ = sc->env_bufs.back()->texels.upload(t0);
+                if (e_ != cudaSuccess) { return fail(PBRT_E_CUDA, std::string("upload light map: ") + cudaGetErrorString(e_)); }
+                sc->upload_bytes += t0.size() * 16;
+                de.texels = sc->env_bufs.back()->texels.p; de.w = pyr[0].us; de.h = pyr[0].vs;
+                lookup_half = mip_lookup(pyr, 0.5f, 0.5f, 0.5f);
+            }
+            const Sp I = mksp(l.L[0], l.L[1], l.L[2]);
+            if (l.kind == PBRT_LIGHT_GONIOMETRIC) sc->h_env_power[i] = lookup_half * I * 4.0f * PB_PI;  // goniometric.rs:266-280
+            else {
+                projection_constants((float)l.env_res[0] / (float)l.env_res[1], l.fov, de.proj, de.screen, de.hither, lights[i].cos_total_width);
+                sc->h_env_power[i] = lookup_half * I * 2.0f * PB_PI * (1.0f - lights[i].cos_total_width);  // projection.rs:379-398
+            }
+            lights[i].env = (uint32_t)envs.size();
+            envs.push_back(de);
         }
         sc->h_lights = lights;
         if (!envs.empty()) UP(envs, envs);
@@ -1672,8 +1736,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                     CK(cudaEventRecord(e, st));
                     k_direct_step<<<(n + 127) / 128, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, iter == 0 ? 1u : 0u, X.rays.p, d_nrays, d_active, d_err, d_prev);
                     const uint64_t total = (uint64_t)n * n_nee;
-                    k_direct_nee<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays,
-                                                                               sc->counters.p, d_err, d_prev);
+                    const unsigned nee_grid = (unsigned)((total + 127) / 128);
+                    if (sc->light_level >= 2) k_direct_nee<2><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
+                    else k_direct_nee<1><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
                     CK(cudaEventRecord(g, st));
                     sev.push_back(e); sev.push_back(g);
                     launches += 2;
@@ -1803,7 +1868,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         const bool plan_instanced = sc->d.n_instances > 0;
         struct ShadeLaunch { int spec; uint32_t lo, hi; };
         std::vector<ShadeLaunch> shade_plan;
-        {
+        if (sc->light_level >= 2) shade_plan.push_back({0, 1u, (uint32_t)PB_SHADE_CLASSES});
+        else {
             uint32_t mask = sc->class_mask & ~1u, covered = 0;
             const uint32_t first_general = PB_SPEC_PLASTIC + 1;
             for (uint32_t c = 1; c < first_general && shade_spec; ++c) {
@@ -1889,6 +1955,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                     else if (l.kind == PBRT_LIGHT_SPOT) pw = I * 2.0f * PB_PI * (1.0f - 0.5f * (l.cos_falloff_start + l.cos_total_width));
                     else if (l.kind == PBRT_LIGHT_DISTANT) pw = I * PB_PI * sc->d.world_radius * sc->d.world_radius;
                     else if (l.kind == PBRT_LIGHT_INFINITE) pw = sc->h_env_power[j] * sp1(PB_PI * sc->d.world_radius * sc->d.world_radius);  // infinite.rs:349-355
+                    else if (l.kind == PBRT_LIGHT_GONIOMETRIC || l.kind == PBRT_LIGHT_PROJECTION) pw = sc->h_env_power[j];
                     else pw = I * (l.two_sided ? 2.0f : 1.0f) * l.area * PB_PI;
                     fixed_f[j] = lum(pw);
                 }
@@ -1931,12 +1998,12 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             int bps = 4;
             cudaError_t oe;
             constexpr int L = 1 + LOBE_LAMBERT;
-            if (halton) oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<false, true, true, L>, PB_SHADE_THREADS, 0)
-                            : sc->area_only ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<true, true, false, L>, PB_SHADE_THREADS, 0)
-                                            : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<false, true, false, L>, PB_SHADE_THREADS, 0);
-            else oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<false, false, true, L>, PB_SHADE_THREADS, shade_smem)
-                     : sc->area_only ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<true, false, false, L>, PB_SHADE_THREADS, shade_smem)
-                                     : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<false, false, false, L>, PB_SHADE_THREADS, shade_smem);
+            if (halton) oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, true, true, L>, PB_SHADE_THREADS, 0)
+                            : sc->light_level == 0 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<0, true, false, L>, PB_SHADE_THREADS, 0)
+                                            : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, true, false, L>, PB_SHADE_THREADS, 0);
+            else oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, false, true, L>, PB_SHADE_THREADS, shade_smem)
+                     : sc->light_level == 0 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<0, false, false, L>, PB_SHADE_THREADS, shade_smem)
+                                     : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, false, false, L>, PB_SHADE_THREADS, shade_smem);
             CK(oe);
             shade_grid_spec = sm_count * std::max(1, std::max(bps, 1) / n_ctx);
         }
@@ -2085,7 +2152,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 launches++;
             }
             if (spatial) {
-                k_lightgrid_contrib<<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
+                if (sc->light_level >= 2) k_lightgrid_contrib<2><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
+                else k_lightgrid_contrib<1><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
                 k_lightgrid_build<<<sm_count, 128, 0, s>>>(V.grid);
                 launches += 2;
             }
@@ -2099,23 +2167,31 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
     do {                                                                                                                                      \
         /* instanced scenes take the general-light variants (an instanced scene lit by area lights alone is rare enough) */                   \
         if (halton) {                                                                                                                         \
-            if (instanced) k_shade<false, true, true, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                            \
-            else if (sc->area_only) k_shade<true, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                   \
-            else k_shade<false, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                                     \
+            if (instanced) k_shade<1, true, true, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                            \
+            else if (sc->light_level == 0) k_shade<0, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                   \
+            else k_shade<1, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                                     \
         } else {                                                                                                                              \
-            if (instanced) k_shade<false, false, true, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                  \
-            else if (sc->area_only) k_shade<true, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);         \
-            else k_shade<false, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                           \
+            if (instanced) k_shade<1, false, true, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                  \
+            else if (sc->light_level == 0) k_shade<0, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);         \
+            else k_shade<1, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                           \
         }                                                                                                                                     \
         launches++;                                                                                                                           \
     } while (0)
             for (const ShadeLaunch& sl : shade_plan) {
+                if (sc->light_level >= 2) {  // image lights: only the general instantiation has them (one launch over every class)
+                    if (halton && instanced) k_shade<2, true, true, 0><<<shade_grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
+                    else if (halton) k_shade<2, true, false, 0><<<shade_grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
+                    else if (instanced) k_shade<2, false, true, 0><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
+                    else k_shade<2, false, false, 0><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
+                    launches++;
+                    continue;
+                }
                 switch (sl.spec) {
                     case 1 + LOBE_LAMBERT: PB_SHADE_LAUNCH(1 + LOBE_LAMBERT, shade_grid_spec, sl.lo, sl.hi); break;
 #define PB_SHADE_SOBOL_ONLY(SPEC)                                                                                                                         \
     do {                                                                                                                                                  \
-        if (sc->area_only) k_shade<true, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                   \
-        else k_shade<false, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                                \
+        if (sc->light_level == 0) k_shade<0, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                   \
+        else k_shade<1, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                                \
         launches++;                                                                                                                                       \
     } while (0)
                     case 1 + LOBE_SPEC_REFL: PB_SHADE_SOBOL_ONLY(1 + LOBE_SPEC_REFL); break;

@@ -639,6 +639,43 @@ int pbrt_host_add_light_distant(PbrtHost* h, const float from[3], const float to
     h->built = false;
     return 0;
 }
+// LightSource "goniometric" / "projection" (api.rs:846-885): light_to_world = the CTM at the directive, I * scale, the map of "mapname"
+// as new_hdr hands it to MipMap::new (rows as the file stores them), and for the projection light "fov".  A goniometric light without a
+// map keeps scale 1; a projection light without one is black in the reference, and comes here as a point light with I = 0.
+static int add_image_light(PbrtHost* h, uint32_t kind, const float I[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
+                           const float* light_to_world, const float* world_to_light, float fov) {
+    if (!h || !I || !light_to_world || !world_to_light) return hfail(PBRT_E_INVALID, "null argument");
+    if (texels && (width == 0 || height == 0)) return hfail(PBRT_E_INVALID, "empty light map");
+    PbrtLight l;
+    std::memset(&l, 0, sizeof l);
+    l.kind = kind;
+    scaled_spectrum(I, scale, l.L);
+    const float* m = light_to_world;  // p_light = light_to_world.transform_point(origin)
+    l.p[0] = m[3]; l.p[1] = m[7]; l.p[2] = m[11];
+    if (m[15] != 1.0f) { const float inv = 1.0f / m[15]; for (int k = 0; k < 3; ++k) l.p[k] = inv * l.p[k]; }
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) l.w2l[3 * i + j] = world_to_light[4 * i + j];
+    auto map = std::make_shared<std::vector<float>>();
+    if (texels) {
+        map->assign(texels, texels + 3 * (size_t)width * height);
+        l.env_res[0] = width; l.env_res[1] = height;
+        l.env_texels = map->data();
+    }
+    l.fov = fov;
+    l.n_samples = h->light_samples;
+    h->light_decls.push_back({h->meshes.size(), l, map});
+    h->built = false;
+    return 0;
+}
+int pbrt_host_add_light_goniometric(PbrtHost* h, const float I[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
+                                    const float light_to_world[16], const float world_to_light[16]) {
+    return add_image_light(h, PBRT_LIGHT_GONIOMETRIC, I, scale, texels, width, height, light_to_world, world_to_light, 0.0f);
+}
+int pbrt_host_add_light_projection(PbrtHost* h, const float I[3], const float scale[3], const float* texels, uint32_t width, uint32_t height, float fov,
+                                   const float light_to_world[16], const float world_to_light[16]) {
+    if (!texels) return hfail(PBRT_E_INVALID, "a projection light without a map is a black point light");
+    return add_image_light(h, PBRT_LIGHT_PROJECTION, I, scale, texels, width, height, light_to_world, world_to_light, fov);
+}
 int pbrt_host_add_light_infinite(PbrtHost* h, const float L[3], const float scale[3], const float* texels, uint32_t width, uint32_t height,
                                  const float* light_to_world, const float* world_to_light) {
     if (!h || !L) return hfail(PBRT_E_INVALID, "null argument");

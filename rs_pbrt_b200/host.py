@@ -174,6 +174,33 @@ class HostScene:
             mi = mi.reshape(-1)
         self._ck(self.L.pbrt_host_add_light_infinite(self.h, _fptr(l), _fptr(sc), _fptr(t), w, h, _fptr(m), _fptr(mi)))
 
+    def _image_light(self, kind, I, scale, texels, light_to_world, world_to_light, fov=None):
+        i, sc = _f32(I), _f32(scale)
+        m = np.array(light_to_world if light_to_world is not None else np.eye(4), np.float64).reshape(4, 4)
+        mi = np.linalg.inv(m) if world_to_light is None else np.array(world_to_light, np.float64).reshape(4, 4)
+        m, mi = _f32(m), _f32(mi)
+        self.log.append((kind, dict(I=i.copy(), scale=None if sc is None else sc.copy(), texels=None if texels is None else np.array(texels, np.float32),
+                                    light_to_world=m.copy(), world_to_light=mi.copy(), fov=fov)))
+        w = h = 0
+        t = None
+        if texels is not None:
+            t = _f32(texels)
+            h, w = t.shape[0], t.shape[1]
+            t = t.reshape(-1)
+        if kind == "light_goniometric":
+            self._ck(self.L.pbrt_host_add_light_goniometric(self.h, _fptr(i), _fptr(sc), _fptr(t), w, h, _fptr(m.reshape(-1)), _fptr(mi.reshape(-1))))
+        else:
+            self._ck(self.L.pbrt_host_add_light_projection(self.h, _fptr(i), _fptr(sc), _fptr(t), w, h, float(fov), _fptr(m.reshape(-1)), _fptr(mi.reshape(-1))))
+
+    def light_goniometric(self, I, scale=None, texels=None, light_to_world=None, world_to_light=None):
+        """LightSource "goniometric": texels = (h, w, 3) map with row 0 first as the .hdr stores it (None: no "mapname");
+        light_to_world = the 4x4 CTM (world_to_light: its inverse, computed in float64 when not given)."""
+        self._image_light("light_goniometric", I, scale, texels, light_to_world, world_to_light)
+
+    def light_projection(self, I, texels, scale=None, fov=45.0, light_to_world=None, world_to_light=None):
+        """LightSource "projection" with a map (without one the reference's light is black: add a point light with I = 0 instead)."""
+        self._image_light("light_projection", I, scale, texels, light_to_world, world_to_light, fov=float(fov))
+
     def look_at(self, eye, look, up):
         e, l, u = (_f32(v) for v in (eye, look, up))
         self.log.append(("look_at", dict(eye=e.copy(), look=l.copy(), up=u.copy())))

@@ -254,6 +254,19 @@ def write(h, path, ply_threshold=2000):
                 m4[:3, :3] = a["light_to_world"]
                 s = "AttributeBegin\n  Transform [%s]\n  %s\nAttributeEnd" % (_nums(m4.T), s)
             world.append(s)
+        elif name in ("light_goniometric", "light_projection"):
+            kind = name[len("light_"):]
+            s = 'LightSource "%s" "rgb I" [%s]' % (kind, _nums(a["I"]))
+            if a["scale"] is not None:
+                s += ' "rgb scale" [%s]' % _nums(a["scale"])
+            if kind == "projection":
+                s += ' "float fov" [%r]' % a["fov"]
+            if a["texels"] is not None:  # rows as the light hands them to MipMap::new: the file's first row is row 0
+                fn = "%s_%s%d.hdr" % (stem, kind, len(world))
+                write_hdr(path.parent / fn, np.asarray(a["texels"], np.float32))
+                notes.append("%s light map %s: written as Radiance RGBE (8-bit mantissas)" % (kind, fn))
+                s += ' "string mapname" ["%s"]' % fn
+            world.append("AttributeBegin\n  Transform [%s]\n  %s\nAttributeEnd" % (_nums(np.asarray(a["light_to_world"], np.float32).T), s))
         elif name == "look_at":
             look = "LookAt %s  %s  %s" % (_nums(a["eye"]), _nums(a["look"]), _nums(a["up"]))
         elif name == "transform_times":

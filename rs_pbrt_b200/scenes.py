@@ -34,6 +34,51 @@ def _box(corners_bottom, height_pts):
     return np.array(idx, np.uint32), P
 
 
+def gonio_map(w=48, h=24, seed=5):
+    """A measured-luminaire stand-in for LightSource "goniometric": (h, w, 3), theta down the rows, phi across, smooth in theta with a
+    phi-dependent lobe and a little noise, so that the swap of y and z, the phi seam and the row order all show in the image."""
+    rng = np.random.default_rng(seed)
+    th = (np.arange(h) + 0.5) / h * np.pi
+    ph = (np.arange(w) + 0.5) / w * 2.0 * np.pi
+    base = 0.3 + 0.7 * np.outer(np.sin(th) ** 2, 0.6 + 0.4 * np.cos(ph))
+    img = np.stack([base, base * (0.8 + 0.2 * np.cos(th))[:, None], base * 0.7], axis=2) * (0.9 + 0.2 * rng.random((h, w, 1)))
+    return img.astype(np.float32)
+
+
+def projector_slide(w=40, h=24, seed=9):
+    """A non-square slide for LightSource "projection": coloured bars and a bright corner marker (its rows as the .hdr stores them)."""
+    rng = np.random.default_rng(seed)
+    img = np.zeros((h, w, 3), np.float32)
+    img[..., 0] = (np.arange(w)[None, :] // 5 % 2) * 0.8 + 0.1
+    img[..., 1] = (np.arange(h)[:, None] // 4 % 2) * 0.7 + 0.2
+    img[..., 2] = 0.3 + 0.4 * rng.random((h, w))
+    img[:4, :6] = 2.0
+    return img
+
+
+def gonio_transform(pos, angle_x=35.0, angle_y=20.0):
+    """CTM of a goniometric light at `pos`, turned about x and y (row-major 4x4, float64)."""
+    ax, ay = np.radians(angle_x), np.radians(angle_y)
+    rx = np.array([[1, 0, 0], [0, np.cos(ax), -np.sin(ax)], [0, np.sin(ax), np.cos(ax)]])
+    ry = np.array([[np.cos(ay), 0, np.sin(ay)], [0, 1, 0], [-np.sin(ay), 0, np.cos(ay)]])
+    m = np.eye(4)
+    m[:3, :3] = ry @ rx
+    m[:3, 3] = pos
+    return m
+
+
+def projector_transform(pos, target, up=(0.0, 1.0, 0.0)):
+    """CTM of a projection light at `pos` whose +z looks at `target` (row-major 4x4, float64)."""
+    z = np.asarray(target, np.float64) - np.asarray(pos, np.float64)
+    z /= np.linalg.norm(z)
+    x = np.cross(np.asarray(up, np.float64), z)
+    x /= np.linalg.norm(x)
+    y = np.cross(z, x)
+    m = np.eye(4)
+    m[:3, 0], m[:3, 1], m[:3, 2], m[:3, 3] = x, y, z, pos
+    return m
+
+
 def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filter="box", xwidth=0.5, ywidth=0.5, lensradius=0.0,
                 focaldistance=1e6, n_threads=8, crop=None, materials="matte", lights="area", sampler="sobol", samplepixelcenter=False, integrator="path", textures=None, lightsamples=1,
                 alpha=None, quantize_textures=False, camera_end=None, shutter=(0.0, 1.0), transform_times=(0.0, 1.0)):
@@ -41,7 +86,8 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
     the spatial light distribution is active).  32 triangles.  `materials="mixed"` swaps the blocks to glass /
     metal and the floor to plastic for BxDF coverage ("translucent", "mix": TranslucentMaterial / MixMaterial on blocks, floor and back wall).  `lights`: "area" (the ceiling quad only), "delta" (plus a point, a spot
     and a distant LightSource, declared before / between / after the shapes so the scene.lights order is interleaved),
-    "point" / "spot" / "distant" (that single delta light and no emitter).  `textures`: None, "ewa" or "trilinear" -- image textures
+    "point" / "spot" / "distant" (that single delta light and no emitter), "goniometric" (a turned goniometric light with
+    gonio_map() under the ceiling, no emitter) or "projection" (a projector throwing the non-square projector_slide() onto the back wall, no emitter).  `textures`: None, "ewa" or "trilinear" -- image textures
     (imagemap.rs) on the floor (matte Kd: a checker of a non-power-of-two resolution, repeated), the back wall (matte Kd: noise,
     clamped, with a uv offset), the short block (plastic Kd and Ks) and the tall block (uber Kd and opacity, some texels opaque
     black / fully transparent so that the lobe list changes from hit to hit).  `alpha`: None, or "masks" -- three cards hang in the box with
@@ -175,6 +221,10 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
                    emit=[17.0, 12.0, 4.0] if lights in ("area", "delta") else None)
     if lights in ("delta", "distant"):
         h.light_distant([0.3, 1.0, -1.5], [0.0, 0.0, 0.0], [1.5, 1.4, 1.1])  # shines in through the open front
+    if lights == "goniometric":
+        h.light_goniometric([30000.0, 28000.0, 24000.0], scale=[1.5, 1.5, 1.5], texels=gonio_map(), light_to_world=gonio_transform([278.0, 470.0, 279.5]))
+    if lights == "projection":
+        h.light_projection([60000.0, 60000.0, 60000.0], projector_slide(), fov=30.0, light_to_world=projector_transform([278.0, 300.0, 20.0], [300.0, 250.0, 555.0]))
     h.look_at([278, 273, -800], [278, 273, 0], [0, 1, 0])
     _camera_motion(h, camera_end, transform_times)
     h.film(xres, yres, crop=crop, filter=filter, xwidth=xwidth, ywidth=ywidth)
@@ -362,11 +412,12 @@ def _fbm(u, v, rng, octaves=6):
 
 
 def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, with_normals=True, n_threads=8, crop=None, integrator="path",
-           dolly=0.0):
+           dolly=0.0, extra_light=None):
     """Ganesha stand-in (config C3): an fBm-displaced, vertically stretched UV sphere of 2*n_side^2 triangles
     (n_side=1468 -> 4.31 M) with per-vertex normals, on a ground quad, lit by 3 rectangular area lights
     (6 light triangles); matte statue + plastic ground.  `dolly` != 0: the camera moves that far towards the statue over the
-    shutter interval (motion blur)."""
+    shutter interval (motion blur).  `extra_light`: None, "point" or "goniometric" -- one more light at the same place above the statue
+    (the goniometric one turned, with gonio_map()): what the image lookup of a goniometric light costs."""
     rng = np.random.default_rng(seed)
     h = HostScene()
     body = h.material(_abi.MAT_MATTE, [0.62, 0.47, 0.33, 0.0])
@@ -408,6 +459,10 @@ def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, wi
     for (cx, cy, cz, sx, sz, L) in [(-3.0, 7.0, -2.0, 1.5, 1.0, [40, 36, 30]), (3.5, 6.0, 1.0, 1.0, 1.5, [18, 22, 30]), (0.0, 8.0, 4.0, 2.0, 0.8, [25, 25, 25])]:
         h.trianglemesh(*_quad([cx - sx, cy, cz - sz], [cx + sx, cy, cz - sz], [cx + sx, cy, cz + sz], [cx - sx, cy, cz + sz]), material=lm,
                        emit=[float(t) for t in L])
+    if extra_light == "point":
+        h.light_point([1.0, 6.5, -3.0], [30.0, 28.0, 24.0])
+    elif extra_light == "goniometric":
+        h.light_goniometric([30.0, 28.0, 24.0], texels=gonio_map(), light_to_world=gonio_transform([1.0, 6.5, -3.0]))
     h.look_at([0.0, 3.2, -7.5], [0.0, 2.0, 0.0], [0, 1, 0])
     if dolly:
         eye = np.array([0.0, 3.2, -7.5]) + dolly * np.array([0.0, -1.2, 7.5]) / np.linalg.norm([0.0, -1.2, 7.5])
