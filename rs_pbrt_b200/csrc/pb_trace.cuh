@@ -567,6 +567,27 @@ PB_D void trace_rays(const DScene& sc, const float4* __restrict__ nodes, const f
 #define PB_WIDE_STACK_ENTRIES 16  // two words per entry: the shared-memory budget of the 32-entry narrow stack
 #endif
 #define PB_WIDE_LEAF_SHIFT 28
+// PB_TRACE_PHASE_CLOCKS (diagnostic builds only, tools/build_variants.py): lane 0 of every trace_rays_wide warp sums the clock64() cycles
+// of the ray refill, the node phase and the leaf phase (the retire stores fall outside all three), and counts the rounds in which some lane
+// held a leaf; every lane counts its triangle tests.  render_impl prints and clears the totals after each render.
+#ifdef PB_TRACE_PHASE_CLOCKS
+__device__ unsigned long long g_trace_phase[5];  // refill, node, leaf cycles; leaf rounds; triangle tests
+#define PB_PHASE_DECL() unsigned long long ph_[5] = {0, 0, 0, 0, 0}; long long ph_t = clock64()
+#define PB_PHASE_START() (ph_t = clock64())
+#define PB_PHASE_LAP(i) do { const long long n_ = clock64(); ph_[i] += (unsigned long long)(n_ - ph_t); ph_t = n_; } while (0)
+#define PB_PHASE_COUNT(i, n) (ph_[i] += (n))
+#define PB_PHASE_FLUSH()                                                                                        \
+    do {                                                                                                        \
+        if (lane == 0) for (int i_ = 0; i_ < 4; ++i_) atomicAdd(&g_trace_phase[i_], ph_[i_]);                   \
+        if (ph_[4]) atomicAdd(&g_trace_phase[4], ph_[4]);                                                       \
+    } while (0)
+#else
+#define PB_PHASE_DECL() do {} while (0)
+#define PB_PHASE_START() do {} while (0)
+#define PB_PHASE_LAP(i) do {} while (0)
+#define PB_PHASE_COUNT(i, n) do {} while (0)
+#define PB_PHASE_FLUSH() do {} while (0)
+#endif
 template <bool INST>
 PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, const float4* __restrict__ tris, const TraceIO& io, uint32_t n_rays,
                           uint32_t* __restrict__ cursor, DCounters* cnt, int walk_steps) {
@@ -634,7 +655,9 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
             else cur = nxt;                                                                                     \
         }                                                                                                       \
     } while (0)
+    PB_PHASE_DECL();
     for (;;) {
+        PB_PHASE_START();
         unsigned idle = __ballot_sync(FULL, !active);
         bool done = false;
         if (idle && !exhausted) {
@@ -662,6 +685,7 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
             }
         }
         if (!__any_sync(FULL, active)) break;
+        PB_PHASE_LAP(0);
         // ---- node phase ---------------------------------------------------------------------------
         for (int step = 0; step < walk_steps; ++step) {  // record visits per lane and round (each covers two tree levels)
             if (!(active && !done && leaf_n == 0u)) break;
@@ -680,12 +704,19 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
             if (!hn && !hf) PB_WPOP();
             PB_WGOTO();
         }
+        PB_PHASE_LAP(1);
+#ifdef PB_TRACE_PHASE_CLOCKS
+        if (__any_sync(FULL, active && leaf_n)) PB_PHASE_COUNT(3, 1);
+#endif
         // ---- leaf phase ----------------------------------------------------------------------------
         if (active && leaf_n) {
             bool entered = false;
             for (uint32_t i = 0; i < leaf_n; ++i) {
+                // Plain scenes load triangles through L1 (no L1::no_allocate): on the H100 that made k_trace 3-4 % shorter on both the
+                // statue and the conference scene (DESIGN.md §7) -- rays traced close together test the same leaves.  The instanced kernel
+                // keeps the streaming hint; it was not measured without it.
                 const float4* tp = tris + 3 * (size_t)(leaf_off + i);
-                const float4 a = ldg4_stream(tp), b = ldg4_stream(tp + 1), c = ldg4_stream(tp + 2);
+                const float4 a = INST ? ldg4_stream(tp) : __ldg(tp), b = INST ? ldg4_stream(tp + 1) : __ldg(tp + 1), c = INST ? ldg4_stream(tp + 2) : __ldg(tp + 2);
                 if (INST && (__float_as_uint(c.w) & TRI_INSTANCE)) {
                     // TransformedPrimitive::intersect / intersect_p (primitive.rs:216-261): the rest of this leaf waits on the stack
                     // under a sentinel, the ray goes into the object's tree in object space
@@ -726,6 +757,7 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
                     break;
                 }
                 THit h;
+                PB_PHASE_COUNT(4, 1);
                 if (tri_test(mk3(a.x, a.y, a.z), mk3(a.w, b.x, b.y), mk3(b.z, b.w, c.x), r, t_max, h)) {
                     t_max = h.t;
                     best = h;
@@ -746,6 +778,7 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
                 }
             }
         }
+        PB_PHASE_LAP(2);
         // ---- retire ----------------------------------------------------------------------------------
         if (active && done) {
             // INST, closest hit: the reference reports a hit only when some primitive RETURNED true (an identity instance does not)
@@ -763,6 +796,7 @@ PB_D void trace_rays_wide(const DScene& sc, const float4* __restrict__ wide, con
 #undef PB_WPOP
 #undef PB_WGOTO
 #undef PB_WPUSH
+    PB_PHASE_FLUSH();
     uint32_t a = n_closest, b = n_shadow;
     for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(FULL, a, o); b += __shfl_xor_sync(FULL, b, o); }
     if (lane == 0) {

@@ -615,12 +615,12 @@ struct TraceLauncher {
         smem_bytes = smem ? scene_bytes : 0;
         wide = wide_enabled() && sc->d.wide != nullptr && !count_work && !alpha && !smem;
         // record visits per lane and round before the warp re-synchronises: long walks keep the lanes that already hold a leaf waiting,
-        // which costs more the longer a record fetch takes -- 6 when the records do not fit in L2 (the 4.3 M-triangle statue), 16 when
-        // they do (the conference scene); PB_WIDE_WALK overrides
+        // which costs more the longer a record fetch takes -- 8 when the records do not fit in L2 (the 4.3 M-triangle statue: 4, 6, 7, 9
+        // and 10 were slower on the H100, DESIGN.md §7), 16 when they do (the conference scene); PB_WIDE_WALK overrides
         {
             int l2 = 0;
             cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, sc->device);
-            wide_walk = (size_t)sc->d.n_nodes * 64 > (size_t)std::max(l2, 1) ? 6 : 16;
+            wide_walk = (size_t)sc->d.n_nodes * 64 > (size_t)std::max(l2, 1) ? 8 : 16;
             if (const char* e_ = getenv("PB_WIDE_WALK")) wide_walk = std::min(64, std::max(1, atoi(e_)));
         }
         int bps = 1;
@@ -2324,6 +2324,16 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         stats->trace_launches = trace_launches;
         stats->kernel_launches = launches;
     }
+#ifdef PB_TRACE_PHASE_CLOCKS
+    {
+        unsigned long long ph[5] = {0, 0, 0, 0, 0};
+        const unsigned long long zero[5] = {0, 0, 0, 0, 0};
+        CK(cudaMemcpyFromSymbol(ph, g_trace_phase, sizeof ph));
+        CK(cudaMemcpyToSymbol(g_trace_phase, zero, sizeof zero));
+        fprintf(stderr, "PB_TRACE_PHASE {\"refill_cycles\": %llu, \"node_cycles\": %llu, \"leaf_cycles\": %llu, \"leaf_rounds\": %llu, \"tri_tests\": %llu}\n",
+                ph[0], ph[1], ph[2], ph[3], ph[4]);
+    }
+#endif
     since("stats + event teardown");
     return PBRT_OK;
 }
