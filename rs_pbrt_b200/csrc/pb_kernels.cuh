@@ -392,9 +392,9 @@ __global__ void __launch_bounds__(256) k_wide_build(const float4* __restrict__ n
     o[3] = make_float4(__uint_as_float(ref[0]), __uint_as_float(ref[1]), __uint_as_float((meta >> 16) & 3u), 0.0f);
 }
 // Launch bounds of the wide trace kernels.  Plain scenes: NO minimum-CTA bound -- ptxas then settles on 64 registers (8 CTAs of 128
-// threads per SM) with its best schedule, which beat both a bound of 1 (more registers, fewer CTAs) and a bound of 8 (registers
-// squeezed) on the statue.  PB_WIDE_MIN_BLOCKS > 0 sets a bound for experiments.  Instanced scenes: a bound of 8 (64 registers
-// instead of 80) was the faster choice on the landscape.
+// threads per SM), which beat a bound of 1, a bound of 8 (registers squeezed), and 9 or 10 CTAs with the leaf-only ray state in shared
+// memory (48 registers at 10): those were slower at every L1 size tried, including the same 92 KB of L1 (DESIGN.md §7, §9).
+// PB_WIDE_MIN_BLOCKS > 0 sets a bound for experiments.  Instanced scenes: a bound of 8 (64 registers instead of 80) was the faster choice on the landscape.
 #ifndef PB_WIDE_MIN_BLOCKS
 #define PB_WIDE_MIN_BLOCKS 0
 #endif
