@@ -23,7 +23,7 @@
  * whitted integrators (PbrtRenderParams.direct_strategy); 4 = PbrtStats.shade_slots / shaded_vertices, tile-interleaved rendering
  * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi); within 4, the animated camera
  * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed); within 4, goniometric and projection lights
- * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word).  Structs only ever grow at their end
+ * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word); within 4, pbrt_gpu_scene_create_multi.  Structs only ever grow at their end
  * within a version step, and a zero-initialised new field means "as before".
  */
 #ifndef PBRT_GPU_H
@@ -372,6 +372,15 @@ typedef struct PbrtMotionDesc {
 /* pbrt_gpu_scene_create with a motion description; motion == NULL is pbrt_gpu_scene_create.  A caller detects motion blur support
  * by this symbol. */
 int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out);
+/* The same scene on n_devices devices in one call, for pbrt_gpu_render_multi: out[i] (an array of n_devices handles) is an ordinary
+ * scene on devices[i], which every entry point accepts and pbrt_gpu_scene_destroy frees on its own, in any order.  The description
+ * is validated and the host-side tables are made once; each large array (BVH nodes, triangle records, per-vertex attributes, texture
+ * pyramids) crosses PCIe once in all: device i uploads its 1/n_devices slice and copies the others from their owners over peer
+ * access (NVLink / NVSwitch), or from the host where a pair has none.  n_devices == 1 is pbrt_gpu_scene_create_motion; motion may
+ * be NULL.  Errors: null desc / devices / out, n_devices == 0 or a device listed twice: PBRT_E_INVALID; more than 16 devices:
+ * PBRT_E_UNSUPPORTED; a bad description or device: what pbrt_gpu_scene_create returns.  On any error every out[i] is NULL. */
+int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n_devices,
+                                PbrtScene** out);
 void pbrt_gpu_scene_destroy(PbrtScene* scene);
 /* Optional (ABI v4): page-lock a host array the caller owns -- nodes, tris, a mesh's p / n / s / uv -- so that pbrt_gpu_scene_create
  * DMAs it where it lies (cudaHostRegister, portable across devices); an array that is not pinned is copied through the library's
@@ -379,7 +388,8 @@ void pbrt_gpu_scene_destroy(PbrtScene* scene);
  * sequence has no need for this; one that re-creates it per frame does (557 MB for the 4.3 M-triangle scene). */
 int pbrt_gpu_host_register(const void* ptr, uint64_t bytes);
 int pbrt_gpu_host_unregister(const void* ptr);
-/* bytes copied host->device by pbrt_gpu_scene_create for this scene (bench.py's h2d_bytes_per_step) */
+/* bytes copied host->device by pbrt_gpu_scene_create for this scene (bench.py's h2d_bytes_per_step); for a replica of
+ * pbrt_gpu_scene_create_multi, the bytes its device received from the host (not those it copied from its peers) */
 uint64_t pbrt_gpu_scene_bytes(const PbrtScene* scene);
 
 /* Render the samples of every pixel in pixel_rect ({x0,y0,x1,y1}, a sub-rectangle
@@ -409,7 +419,8 @@ int pbrt_gpu_render_device(PbrtScene* scene, const PbrtRenderParams* params, con
 int pbrt_gpu_render_tiles_device(PbrtScene* scene, const PbrtRenderParams* params, uint32_t part, uint32_t n_parts, float* d_film_rgbw,
                                  void* cuda_stream, PbrtStats* stats);
 /* pbrt_gpu_render_multi: the whole frame on n_scenes devices from ONE process -- what a single rs_pbrt process calls in place of
- * its Rayon tile loop.  scenes[i] is the same description created on device i (pbrt_gpu_scene_create per device; scene replicated).
+ * its Rayon tile loop.  scenes[i] is the same description created on device i (pbrt_gpu_scene_create_multi, or
+ * pbrt_gpu_scene_create per device).
  * One host thread per device renders part i of n_scenes; the device of scenes[0] then sums the other films in ONE pass, reading them
  * through NVLink / NVSwitch peer access (a staged peer copy where a pair has none), and the result is ADDED into the HOST array
  * film_rgbw exactly like pbrt_gpu_render.  stats: counters summed over the devices, times = the slowest device (+ the reduce). */

@@ -5,6 +5,6 @@ this package only holds the ctypes bindings and the synthetic scene generators u
 Importing the package does not load the library; the first call does, and fails loudly if it is missing.
 """
 from . import _abi  # noqa: F401
-from .host import GpuScene, HostScene, PbrtError, bvh_build, pin_description, render_multi, unpin_description  # noqa: F401
+from .host import GpuScene, HostScene, PbrtError, bvh_build, create_multi, pin_description, render_multi, unpin_description  # noqa: F401
 
-__all__ = ["GpuScene", "HostScene", "PbrtError", "bvh_build", "render_multi", "pin_description", "unpin_description"]
+__all__ = ["GpuScene", "HostScene", "PbrtError", "bvh_build", "create_multi", "render_multi", "pin_description", "unpin_description"]

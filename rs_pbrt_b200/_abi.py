@@ -105,7 +105,7 @@ class PbrtStats(C.Structure):
 GPU_SYMBOLS = ["pbrt_gpu_scene_create", "pbrt_gpu_scene_destroy", "pbrt_gpu_scene_bytes", "pbrt_gpu_render", "pbrt_gpu_render_device", "pbrt_gpu_render_samples",
                "pbrt_gpu_render_tiles_device", "pbrt_gpu_render_multi", "pbrt_gpu_host_register", "pbrt_gpu_host_unregister",
                "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2",
-               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate"]
+               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate", "pbrt_gpu_scene_create_multi"]
 HOST_SYMBOLS = ["pbrt_host_new", "pbrt_host_free", "pbrt_host_last_error", "pbrt_host_add_material", "pbrt_host_add_material_mix", "pbrt_host_add_trianglemesh",
                 "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
                 "pbrt_host_integrator_path", "pbrt_host_world_end", "pbrt_host_scene_desc", "pbrt_host_render_params", "pbrt_host_render",
@@ -136,6 +136,7 @@ def bind(L):
     vp = C.c_void_p
     L.pbrt_gpu_scene_create.argtypes = [C.POINTER(PbrtSceneDesc), C.c_int, C.POINTER(vp)]
     L.pbrt_gpu_scene_create_motion.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.c_int, C.POINTER(vp)]
+    L.pbrt_gpu_scene_create_multi.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(C.c_int), C.c_uint32, C.POINTER(vp)]
     L.pbrt_gpu_kat_animated_interpolate.argtypes = [C.c_int, C.POINTER(PbrtAnimatedTransform), C.c_uint32, fp, fp, fp]
     L.pbrt_gpu_scene_destroy.argtypes = [vp]
     L.pbrt_gpu_scene_destroy.restype = None

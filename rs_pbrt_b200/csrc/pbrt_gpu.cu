@@ -468,11 +468,13 @@ struct DeviceScratch {
     // timing events are pooled per device: a frame records four per wavefront iteration, and cudaEventCreate / Destroy of several
     // hundred events was a measurable part of the fixed cost of a render call
     // pbrt_gpu_scene_create: pinned staging for the flattened triangle records (written by the host threads, DMA'd from there while
-    // the next chunk is being flattened) and the two upload streams; stage_mu serialises scene creation per device
+    // the next chunk is being flattened) and the two upload streams; stage_mu serialises scene creation per device.  shard_ev: this
+    // device's slices of a multi-device scene_create have arrived (the other devices copy them from here after it)
     unsigned char* stage = nullptr;
     size_t stage_n = 0;
     cudaStream_t up_stream[2] = {nullptr, nullptr};
     cudaEvent_t slot_ev[2] = {nullptr, nullptr};
+    cudaEvent_t shard_ev = nullptr;
     std::mutex stage_mu;
     bool pool_ready = false;
     cudaError_t staging(size_t bytes) {
@@ -707,25 +709,151 @@ const char* pbrt_gpu_last_error(void) { return g_err.c_str(); }
 int pbrt_gpu_abi_version(void) { return PBRT_GPU_ABI_VERSION; }
 uint64_t pbrt_gpu_launch_count(void) { return g_launches.load(); }
 
-int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out) {
-    if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    static const int timing = getenv("PB_TIMING") ? atoi(getenv("PB_TIMING")) : 0;  // 1: every call; 2: only calls slower than 100 ms
-    const auto t_enter = std::chrono::steady_clock::now();
-    std::string timing_log;
-    auto since = [&](const char* what) {
-        if (!timing) return;
-        char line[160];
-        snprintf(line, sizeof line, "[pb timing] scene_create %-26s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enter).count());
-        if (timing == 1) fputs(line, stderr); else timing_log += line;
-    };
-    struct SlowDump { std::string& log; const std::chrono::steady_clock::time_point t0; int mode; ~SlowDump() {
-        if (mode == 2 && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() > 100.0) fputs(log.c_str(), stderr); } } slow_dump{timing_log, t_enter, timing};
-    *out = nullptr;
+}  // extern "C"
+
+static bool finite_keyframes(const PbrtAnimatedTransform& a) {
+    bool ok = std::isfinite(a.start_time) && std::isfinite(a.end_time);
+    for (int k = 0; k < 16; ++k)
+        ok = ok && std::isfinite(a.start[k]) && std::isfinite(a.start_inv[k]) && std::isfinite(a.end[k]) && std::isfinite(a.end_inv[k]);
+    return ok;
+}
+
+// m_inv is the inverse of m up to f32 rounding: every element of m * m_inv (in f64) lies within 1e-4 of the sum of the magnitudes of
+// its terms of the identity's element.  A caller that hands over another matrix's inverse (or a transposed one) is caught here.
+static bool inverse_pair(const float* m, const float* m_inv) {
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j) {
+            double p = 0.0, mag = 0.0;
+            for (int k = 0; k < 4; ++k) { p += (double)m[4 * i + k] * m_inv[4 * k + j]; mag += std::fabs((double)m[4 * i + k] * m_inv[4 * k + j]); }
+            if (!(std::fabs(p - (i == j ? 1.0 : 0.0)) <= 1e-4 * mag + 1e-6)) return false;
+        }
+    return true;
+}
+
+// Lets `from` read `to`'s memory directly (NVLink / NVSwitch) and leaves `from` the current device.  False where the pair has no peer
+// access or enabling it fails (the sticky error is cleared): the caller then takes its staged path for that pair.
+static bool enable_peer_access(int from, int to) {
+    int can = 0;
+    if (cudaSetDevice(from) != cudaSuccess || cudaDeviceCanAccessPeer(&can, from, to) != cudaSuccess || !can) { cudaGetLastError(); return false; }
+    const cudaError_t e = cudaDeviceEnablePeerAccess(to, 0);
+    if (e == cudaSuccess) return true;
+    cudaGetLastError();
+    return e == cudaErrorPeerAccessAlreadyEnabled;
+}
+
+// ---- scene creation --------------------------------------------------------------------------------------------------------------
+// pbrt_gpu_scene_create, _create_motion and _create_multi are one code path in two phases.  scene_prepare validates the description
+// and makes every host-side table once: lobe lists and shading classes, texture / environment / light-map pyramids and their
+// distributions, light records, Sobol' tables, the BVH depth check.  build_begin / build_finish then make the scene on each device
+// from that state.
+
+// The large arrays: the caller's BVH nodes, triangle records and per-vertex attributes, and the image-texture pyramids.  With n
+// devices each is cut into n contiguous slices of whole elements; device i uploads slice i from the host and copies the others from
+// the devices that uploaded them.
+enum { BIG_TRIS, BIG_P, BIG_NODES, BIG_N, BIG_UV, BIG_S, BIG_TEX0 };  // image texture t is BIG_TEX0 + t (empty for the other kinds)
+struct BigArray {
+    struct Piece { size_t off; const void* src; size_t bytes; };  // bytes [off, off + bytes) of the array are at src
+    size_t bytes = 0, elem = 1;
+    std::vector<Piece> pieces;
+    void slice(uint32_t k, uint32_t n, size_t& lo, size_t& hi) const {  // the byte range of slice k of n
+        const size_t ne = bytes / elem;
+        lo = elem * (ne * k / n);
+        hi = elem * (ne * (k + 1) / n);
+    }
+};
+
+struct ScenePrep {
+    const PbrtSceneDesc* desc = nullptr;
+    std::vector<size_t> vbase;
+    size_t total_verts = 0;
+    bool any_n = false, any_uv = false, any_s = false, any_alpha = false, wide = false;
+    std::vector<DMaterial> mats, mats_single;
+    std::vector<DMatSrc> mat_src;
+    std::vector<DLight> lights;
+    std::vector<Sp> env_power;
+    std::vector<HostEnv> envs;  // one per DEnv: an infinite light's map and Distribution2D, or a light map's level 0
+    std::vector<DEnv> denvs;    // (device pointers filled in per device)
+    std::vector<DMeshRec> meshes;
+    std::vector<DInstance> instances;
+    std::vector<uint2> mesh_alpha;
+    std::vector<DTexture> textures;  // (texel pointers filled in per device)
+    std::vector<std::vector<float4>> tex_texels;
+    std::vector<float> ewa_lut;
+    std::vector<uint32_t> m32, nib;
+    std::vector<uint64_t> vdc, vdci;
+    std::vector<float> halton;
+    std::vector<BigArray> big;
+    DScene d;  // everything but the device pointers
+    int light_level = 0;
+    uint32_t class_mask = 0;
+    DMotion cam_mo;
+};
+
+// The host-side passes run on all cores (a 4.3 M-triangle scene is re-uploaded on every end-to-end step).
+static int parallel_for(uint32_t n, const std::function<int(uint32_t, uint32_t)>& body) {
+    const unsigned nt = n < 65536 ? 1u : host_threads();
+    std::vector<int> rc(nt, 0);
+    std::vector<std::thread> th;
+    for (unsigned t = 0; t < nt; ++t) {
+        uint32_t lo = (uint32_t)((uint64_t)n * t / nt), hi = (uint32_t)((uint64_t)n * (t + 1) / nt);
+        if (nt == 1) rc[0] = body(lo, hi);
+        else th.emplace_back([&, t, lo, hi] { rc[t] = body(lo, hi); });
+    }
+    for (auto& x : th) x.join();
+    for (int r : rc) if (r) return r;
+    return 0;
+}
+
+// The triangle checks: k_flatten_tris makes them on the device, fused with the flattening; tri_error is the same test on the host for
+// a call that has no usable device.
+static int tri_error(const PbrtSceneDesc* desc, const PbrtTri& t) {
+    if (t.mesh == PBRT_MESH_INSTANCE) return t.v[0] >= desc->n_instances ? 5 : 0;
+    if (t.mesh >= desc->n_meshes) return 1;
+    const PbrtMesh& m = desc->meshes[t.mesh];
+    if (t.v[0] >= m.n_verts || t.v[1] >= m.n_verts || t.v[2] >= m.n_verts) return 2;
+    if (t.material != PBRT_NO_MATERIAL && t.material >= desc->n_materials) return 3;
+    if (t.area_light >= (int32_t)desc->n_lights) return 4;
+    if (t.area_light >= 0 && (m.alpha || m.shadow_alpha)) return 6;
+    return 0;
+}
+static int tri_fail(int code) {
+    if (code == 1) return fail(PBRT_E_INVALID, "triangle mesh index out of range");
+    if (code == 2) return fail(PBRT_E_INVALID, "vertex index out of range");
+    if (code == 3) return fail(PBRT_E_INVALID, "material index out of range");
+    if (code == 4) return fail(PBRT_E_INVALID, "area light index out of range");
+    if (code == 6) return fail(PBRT_E_UNSUPPORTED, "alpha mask on an emissive mesh is outside the GPU path (pdf_li would have to evaluate it)");
+    return fail(PBRT_E_INVALID, "instance index out of range");
+}
+
+static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, ScenePrep& P) {
+    P.desc = desc;
+    std::memset(&P.cam_mo, 0, sizeof P.cam_mo);
+    if (motion && motion->instances) {
+        if (desc->n_instances && !desc->instances) return fail(PBRT_E_INVALID, "null instance array in scene description");
+        for (uint32_t i = 0; i < desc->n_instances; ++i) {
+            const PbrtAnimatedTransform& a = motion->instances[i];
+            if (!finite_keyframes(a)) return fail(PBRT_E_UNSUPPORTED, "instance keyframe matrix or time is not finite");
+            if (std::memcmp(a.start, desc->instances[i].m, 64) != 0 || std::memcmp(a.start_inv, desc->instances[i].m_inv, 64) != 0)
+                return fail(PBRT_E_INVALID, "an instance's start keyframe differs from PbrtInstance.m / m_inv");
+            for (int k = 0; k < 16; ++k)
+                if (a.start[k] != a.end[k] || a.start_inv[k] != a.end_inv[k])
+                    return fail(PBRT_E_UNSUPPORTED, "animated object instances are outside the GPU path");
+        }
+    }
+    if (const PbrtAnimatedTransform* c = motion ? motion->camera : nullptr) {
+        if (!finite_keyframes(*c)) return fail(PBRT_E_UNSUPPORTED, "camera keyframe matrix or time is not finite");
+        if (std::memcmp(c->start, desc->camera.camera_to_world, 64) != 0)
+            return fail(PBRT_E_INVALID, "the camera's start keyframe differs from PbrtCamera.camera_to_world");
+        if (!inverse_pair(c->start, c->start_inv) || !inverse_pair(c->end, c->end_inv))
+            return fail(PBRT_E_INVALID, "a camera keyframe's m_inv is not the inverse of its m");
+        motion_create(c->start, c->start_inv, c->start_time, c->end, c->end_inv, c->end_time, P.cam_mo);
+    }
     if ((desc->n_nodes && !desc->nodes) || (desc->n_tris && !desc->tris) || (desc->n_meshes && !desc->meshes) ||
         (desc->n_materials && !desc->materials) || (desc->n_lights && !desc->lights))
         return fail(PBRT_E_INVALID, "null array in scene description");
     // ---- validate + flatten on the host ------------------------------------------------------
-    std::vector<size_t> vbase(desc->n_meshes + 1, 0);
+    std::vector<size_t>& vbase = P.vbase;
+    vbase.assign(desc->n_meshes + 1, 0);
     bool any_n = false, any_uv = false, any_s = false, any_alpha = false;
     for (uint32_t i = 0; i < desc->n_meshes; ++i) {
         const PbrtMesh& m = desc->meshes[i];
@@ -740,8 +868,12 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
         any_n |= m.n != nullptr; any_uv |= m.uv != nullptr; any_s |= m.s != nullptr;
     }
     const size_t total_verts = vbase[desc->n_meshes];
-    std::vector<DMaterial> mats(desc->n_materials);
-    std::vector<DMaterial> mats_single(desc->n_materials);  // the lobe lists without allow_multiple_lobes (DirectLighting / Whitted: directlighting.rs:77)
+    P.total_verts = total_verts;
+    P.any_n = any_n; P.any_uv = any_uv; P.any_s = any_s; P.any_alpha = any_alpha;
+    std::vector<DMaterial>& mats = P.mats;
+    std::vector<DMaterial>& mats_single = P.mats_single;  // the lobe lists without allow_multiple_lobes (DirectLighting / Whitted: directlighting.rs:77)
+    mats.resize(desc->n_materials);
+    mats_single.resize(desc->n_materials);
     for (uint32_t i = 0; i < desc->n_materials; ++i) {
         const char* why = "";
         if (!compile_material_at(desc->materials, desc->n_materials, i, mats[i], true, nullptr, &why) ||
@@ -769,7 +901,8 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     }
     // image textures (ABI v3): the class above is that of the all-constants lobe list; what k_shade runs on comes from k_texture
     if (desc->n_textures && !desc->textures) return fail(PBRT_E_INVALID, "null texture array");
-    std::vector<DMatSrc> mat_src(desc->n_textures ? desc->n_materials : 0);
+    std::vector<DMatSrc>& mat_src = P.mat_src;
+    mat_src.resize(desc->n_textures ? desc->n_materials : 0);
     for (uint32_t i = 0; i < desc->n_materials; ++i) {
         const PbrtMaterial& pm = desc->materials[i];
         bool textured = false;
@@ -824,7 +957,8 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
         } else return fail(PBRT_E_UNSUPPORTED, "texture kind outside the GPU path");
     }
     if (desc->n_instances && !desc->instances) return fail(PBRT_E_INVALID, "null instance array");
-    std::vector<DLight> lights(desc->n_lights);
+    std::vector<DLight>& lights = P.lights;
+    lights.resize(desc->n_lights);
     uint32_t n_inf = 0, inf_idx[PBRT_MAX_INFINITE_LIGHTS] = {0, 0, 0, 0};
     for (uint32_t i = 0; i < desc->n_lights; ++i) {
         const PbrtLight& l = desc->lights[i];
@@ -860,21 +994,7 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
             if (l.kind == PBRT_LIGHT_PROJECTION && !(l.fov > 0.0f && l.fov < 180.0f)) return fail(PBRT_E_INVALID, "projection light fov outside (0, 180) degrees");
         }
     }
-    // The host-side flattening runs on all cores (a 4.3 M-triangle scene is re-uploaded on every end-to-end step).
     const unsigned hw = host_threads();
-    auto parallel_for = [&](uint32_t n, const std::function<int(uint32_t, uint32_t)>& body) -> int {
-        const unsigned nt = n < 65536 ? 1u : hw;
-        std::vector<int> rc(nt, 0);
-        std::vector<std::thread> th;
-        for (unsigned t = 0; t < nt; ++t) {
-            uint32_t lo = (uint32_t)((uint64_t)n * t / nt), hi = (uint32_t)((uint64_t)n * (t + 1) / nt);
-            if (nt == 1) rc[0] = body(lo, hi);
-            else th.emplace_back([&, t, lo, hi] { rc[t] = body(lo, hi); });
-        }
-        for (auto& x : th) x.join();
-        for (int r : rc) if (r) return r;
-        return 0;
-    };
     // BVH nodes: PbrtBvhNode already IS the device layout (32 bytes: 6 floats, offset, n_prims | axis << 16 | pad << 24;
     // the kernels mask the pad byte), so the caller's array is validated in place and uploaded without staging.
     static_assert(sizeof(PbrtBvhNode) == 32, "LinearBVHNode layout");
@@ -893,7 +1013,6 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     });
     if (vrc == 1) return fail(PBRT_E_INVALID, "BVH leaf range out of bounds");
     if (vrc == 2) return fail(PBRT_E_INVALID, "BVH interior node malformed");
-    since("nodes validated");
     {
         // Tree depth: the traversal stack holds 64 entries like the reference's nodes_to_visit (bvh.rs:420,480), one per interior
         // ancestor whose far child is pending; a deeper tree would index past the reference's array (a panic there) and past the
@@ -999,107 +1118,8 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
             }
         }
     }
-    since("depth + instance checks");
-    // ---- device, scene object, and the big uploads ------------------------------------------------------------------------------
-    // The caller's arrays go up as they are -- nodes, triangle records, per-vertex attributes -- and the triangles are validated and
-    // flattened (pre-gathered vertices in BVH order) by a kernel: the host side of a 4.3 M-triangle scene_create is then the node checks.
-    auto tri_error = [&](const PbrtTri& t) -> int {  // what the flattening below rejects
-        if (t.mesh == PBRT_MESH_INSTANCE) return t.v[0] >= desc->n_instances ? 5 : 0;
-        if (t.mesh >= desc->n_meshes) return 1;
-        const PbrtMesh& m = desc->meshes[t.mesh];
-        if (t.v[0] >= m.n_verts || t.v[1] >= m.n_verts || t.v[2] >= m.n_verts) return 2;
-        if (t.material != PBRT_NO_MATERIAL && t.material >= desc->n_materials) return 3;
-        if (t.area_light >= (int32_t)desc->n_lights) return 4;
-        if (t.area_light >= 0 && (m.alpha || m.shadow_alpha)) return 6;
-        return 0;
-    };
-    auto tri_fail = [&](int code) -> int {
-        if (code == 1) return fail(PBRT_E_INVALID, "triangle mesh index out of range");
-        if (code == 2) return fail(PBRT_E_INVALID, "vertex index out of range");
-        if (code == 3) return fail(PBRT_E_INVALID, "material index out of range");
-        if (code == 4) return fail(PBRT_E_INVALID, "area light index out of range");
-        if (code == 6) return fail(PBRT_E_UNSUPPORTED, "alpha mask on an emissive mesh is outside the GPU path (pdf_li would have to evaluate it)");
-        return fail(PBRT_E_INVALID, "instance index out of range");
-    };
-    int rc = check_device(device);
-    if (rc != PBRT_OK) {
-        // no usable device: a malformed description is still reported as such (validation does not depend on the hardware; it is
-        // otherwise fused with the flattening below)
-        const std::string dev_err = g_err;
-        vrc = parallel_for(desc->n_tris, [&](uint32_t lo, uint32_t hi) -> int {
-            for (uint32_t i = lo; i < hi; ++i) if (int e = tri_error(desc->tris[i])) return e;
-            return 0;
-        });
-        if (vrc) return tri_fail(vrc);
-        return fail(rc, dev_err);
-    }
-    DeviceScratch* up_scr = scratch_for(device);
-    if (!up_scr) return fail(PBRT_E_INVALID, "device ordinal out of range");
-    std::unique_lock<std::mutex> stage_lock(up_scr->stage_mu);
-    if (!up_scr->pool_ready) {
-        for (int k = 0; k < 2; ++k) CK(cudaStreamCreateWithFlags(&up_scr->up_stream[k], cudaStreamNonBlocking));
-        for (int k = 0; k < 2; ++k) CK(cudaEventCreateWithFlags(&up_scr->slot_ev[k], cudaEventDisableTiming));
-        up_scr->pool_ready = true;
-    }
-    std::unique_ptr<PbrtScene> sc_guard(new PbrtScene());
-    PbrtScene* sc = sc_guard.get();
-    sc->device = device;
-    sc->recycle_buffers(device);
-    DevBuf<uint2> raw_tris;   // the caller's PbrtTri records as they are (24 B each), flattened on the device
-    DevBuf<float> raw_p;      // mesh positions, concatenated
-    DevBuf<DMeshRec> d_meshes;
-    DevBuf<uint32_t> d_status;
-    raw_tris.cache_dev = raw_p.cache_dev = d_meshes.cache_dev = d_status.cache_dev = device;
-    CK(sc->nodes.alloc(2 * (size_t)desc->n_nodes));
-    CK(sc->tri_verts.alloc(3 * (size_t)desc->n_tris));
-    CK(sc->tri_idx.alloc((size_t)desc->n_tris));
-    CK(raw_tris.alloc(3 * (size_t)desc->n_tris));
-    CK(raw_p.alloc(3 * total_verts));
-    if (any_n) CK(sc->vn.alloc(3 * total_verts));
-    if (any_uv) CK(sc->vuv.alloc(2 * total_verts));
-    if (any_s) CK(sc->vs.alloc(3 * total_verts));
-    CK(d_meshes.alloc(std::max<size_t>(desc->n_meshes, 1)));
-    CK(d_status.alloc(2));
-    since("device buffers allocated");
-    // ---- uploads.  A source array in pinned memory (the caller's own cudaHostAlloc / pbrt_gpu_host_register) is DMA'd where it
-    // lies; pageable memory goes through two pinned staging slots, copied into them on all cores while the previous slot is in flight
-    // (a cudaMemcpy straight from pageable memory runs at a fraction of the pinned rate).
-    cudaStream_t ups = up_scr->up_stream[1];
-    const size_t slot_bytes = (size_t)64 << 20;
-    CK(up_scr->staging(2 * slot_bytes));
-    cudaEvent_t* const slot_ev = up_scr->slot_ev;
-    bool slot_used[2] = {false, false};
-    int next_slot = 0;
-    size_t up_bytes = 0;
-    auto upload = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
-        if (!bytes) return cudaSuccess;
-        up_bytes += bytes;
-        cudaPointerAttributes at;
-        const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
-        cudaGetLastError();
-        if (pinned) return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ups);
-        for (size_t off = 0; off < bytes; off += slot_bytes) {
-            const size_t n = std::min(slot_bytes, bytes - off);
-            const int k = next_slot;
-            next_slot ^= 1;
-            if (slot_used[k]) { cudaError_t e = cudaEventSynchronize(slot_ev[k]); if (e != cudaSuccess) return e; }
-            unsigned char* stage = up_scr->stage + (size_t)k * slot_bytes;
-            const unsigned char* from = static_cast<const unsigned char*>(src) + off;
-            if (n < ((size_t)1 << 20)) std::memcpy(stage, from, n);
-            else {
-                const unsigned nt = hw;
-                std::vector<std::thread> th;
-                for (unsigned t = 0; t < nt; ++t) th.emplace_back([=] { const size_t lo = n * t / nt, hi = n * (t + 1) / nt; std::memcpy(stage + lo, from + lo, hi - lo); });
-                for (auto& x : th) x.join();
-            }
-            cudaError_t e = cudaMemcpyAsync(static_cast<unsigned char*>(dst) + off, stage, n, cudaMemcpyHostToDevice, ups);
-            if (e == cudaSuccess) e = cudaEventRecord(slot_ev[k], ups);
-            if (e != cudaSuccess) return e;
-            slot_used[k] = true;
-        }
-        return cudaSuccess;
-    };
-    std::vector<DMeshRec> h_meshes(std::max<size_t>(desc->n_meshes, 1));
+    if (total_verts >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "more than 2^32 vertices");
+    P.meshes.resize(std::max<size_t>(desc->n_meshes, 1));
     for (uint32_t i = 0; i < desc->n_meshes; ++i) {
         const PbrtMesh& m = desc->meshes[i];
         uint32_t flags = 0;
@@ -1109,54 +1129,18 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
         if (m.s) flags |= TRI_HAS_S;
         if (m.alpha) flags |= TRI_ALPHA;
         if (m.shadow_alpha) flags |= TRI_SHADOW_ALPHA;
-        h_meshes[i].vbase = (uint32_t)vbase[i]; h_meshes[i].n_verts = m.n_verts; h_meshes[i].flags = flags; h_meshes[i].pad = 0;
+        P.meshes[i].vbase = (uint32_t)vbase[i]; P.meshes[i].n_verts = m.n_verts; P.meshes[i].flags = flags; P.meshes[i].pad = 0;
     }
-    if (total_verts >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "more than 2^32 vertices");
-    {
-        cudaError_t e = cudaMemcpyAsync(d_meshes.p, h_meshes.data(), h_meshes.size() * sizeof(DMeshRec), cudaMemcpyHostToDevice, ups);
-        if (e == cudaSuccess) e = cudaMemsetAsync(d_status.p, 0, 8, ups);
-        if (e == cudaSuccess) e = upload(raw_tris.p, desc->tris, 24 * (size_t)desc->n_tris);
-        for (uint32_t i = 0; i < desc->n_meshes && e == cudaSuccess; ++i) {
-            const PbrtMesh& m = desc->meshes[i];
-            e = upload(raw_p.p + 3 * vbase[i], m.p, 12 * (size_t)m.n_verts);
-        }
-        if (e != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload triangles / positions: ") + cudaGetErrorString(e));
-        // triangles: validated and pre-gathered (vertices in BVH order) on the device
-        if (desc->n_tris) {
-            k_flatten_tris<<<(desc->n_tris + 255) / 256, 256, 0, ups>>>(raw_tris.p, desc->n_tris, d_meshes.p, desc->n_meshes, raw_p.p, desc->n_materials, desc->n_lights,
-                                                                       desc->n_instances, sc->tri_verts.p, sc->tri_idx.p, d_status.p);
-            g_launches++;
-        }
-        e = upload(sc->nodes.p, desc->nodes, 32 * (size_t)desc->n_nodes);
-        // per-vertex attributes go from the caller's mesh arrays into the concatenated device arrays
-        for (uint32_t i = 0; i < desc->n_meshes && e == cudaSuccess; ++i) {
-            const PbrtMesh& m = desc->meshes[i];
-            if (m.n) e = upload(sc->vn.p + 3 * vbase[i], m.n, 12 * (size_t)m.n_verts);
-            if (e == cudaSuccess && m.uv) e = upload(sc->vuv.p + 2 * vbase[i], m.uv, 8 * (size_t)m.n_verts);
-            if (e == cudaSuccess && m.s) e = upload(sc->vs.p + 3 * vbase[i], m.s, 12 * (size_t)m.n_verts);
-        }
-        if (e != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload nodes / vertex attributes: ") + cudaGetErrorString(e));
-    }
-    since("uploads queued");
-    uint32_t h_status[2] = {0, 0};
-    CK(cudaMemcpyAsync(h_status, d_status.p, 8, cudaMemcpyDeviceToHost, ups));
-    CK(cudaStreamSynchronize(ups));  // (the staging slots and the temporaries are quiet from here on)
-    CK(cudaGetLastError());
-    vrc = (int)h_status[0];
-    std::atomic<int> null_seen((int)h_status[1]);
-    if (vrc) return tri_fail(vrc);
-    std::vector<DInstance> dinst(desc->n_instances);
+    P.instances.resize(desc->n_instances);
     for (uint32_t i = 0; i < desc->n_instances; ++i) {
         const PbrtInstance& I = desc->instances[i];
-        if (I.root >= desc->n_nodes) return fail(PBRT_E_INVALID, "instance root out of range");
-        std::memset(&dinst[i], 0, sizeof(DInstance));
-        dinst[i].root = I.root;
-        dinst[i].identity = I.identity ? 1u : 0u;
-        std::memcpy(dinst[i].m, I.m, 64);
-        std::memcpy(dinst[i].m_inv, I.m_inv, 64);
+        DInstance& di = P.instances[i];
+        std::memset(&di, 0, sizeof(DInstance));
+        di.root = I.root;
+        di.identity = I.identity ? 1u : 0u;
+        std::memcpy(di.m, I.m, 64);
+        std::memcpy(di.m_inv, I.m_inv, 64);
     }
-    const bool has_null = null_seen.load() != 0;
-    since("triangles flattened");
     // ---- Sobol' tables (embedded blob) ---------------------------------------------------------
     const unsigned char* blob = pb_sobol_blob_start;
     size_t blob_size = (size_t)(pb_sobol_blob_end - pb_sobol_blob_start);
@@ -1165,127 +1149,86 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
     if (blob_size < need) return fail(PBRT_E_INVALID, "embedded Sobol table blob truncated");
     std::memcpy(hdr, blob, 32);
     if (hdr[0] != 0x4C424F53u || hdr[1] != 1024 || hdr[2] != 52) return fail(PBRT_E_INVALID, "embedded Sobol table blob corrupt");
-    std::vector<uint32_t> m32(1024 * 52);
-    std::vector<uint64_t> vdc(25 * 52), vdci(26 * 52);
-    std::memcpy(m32.data(), blob + 32, m32.size() * 4);
-    std::memcpy(vdc.data(), blob + 32 + m32.size() * 4, vdc.size() * 8);
-    std::memcpy(vdci.data(), blob + 32 + m32.size() * 4 + vdc.size() * 8, vdci.size() * 8);
+    P.m32.resize(1024 * 52);
+    P.vdc.resize(25 * 52);
+    P.vdci.resize(26 * 52);
+    std::memcpy(P.m32.data(), blob + 32, P.m32.size() * 4);
+    std::memcpy(P.vdc.data(), blob + 32 + P.m32.size() * 4, P.vdc.size() * 8);
+    std::memcpy(P.vdci.data(), blob + 32 + P.m32.size() * 4 + P.vdc.size() * 8, P.vdci.size() * 8);
     // nibble tables nib[dim][chunk][e] (pb_sobol.cuh)
-    std::vector<uint32_t> nib((size_t)1024 * PB_SOBOL_CHUNKS * 16);
+    P.nib.resize((size_t)1024 * PB_SOBOL_CHUNKS * 16);
     for (int dim = 0; dim < 1024; ++dim)
         for (int c = 0; c < PB_SOBOL_CHUNKS; ++c)
             for (int e = 0; e < 16; ++e) {
                 uint32_t v = 0;
                 for (int j = 0; j < 4; ++j)
-                    if (e & (1 << j)) v ^= m32[(size_t)dim * 52 + 4 * c + j];
-                nib[((size_t)dim * PB_SOBOL_CHUNKS + c) * 16 + e] = v;
+                    if (e & (1 << j)) v ^= P.m32[(size_t)dim * 52 + 4 * c + j];
+                P.nib[((size_t)dim * PB_SOBOL_CHUNKS + c) * 16 + e] = v;
             }
-    std::vector<float> halton(128 * 5);
+    P.halton.resize(128 * 5);
     for (int s = 0; s < 128; ++s)
-        for (int k = 0; k < 5; ++k) halton[5 * s + k] = host_radical_inverse(k, (uint64_t)s);
-
-    since("tables built");
-    sc->has_null_material = has_null;
-    sc->h_nib = nib;
-    for (const DLight& l : lights) sc->light_level = std::max(sc->light_level, l.kind == PBRT_LIGHT_DIFFUSE_AREA ? 0 : l.kind < PBRT_LIGHT_GONIOMETRIC ? 1 : 2);
-    for (const DMaterial& m : mats) sc->class_mask |= 1u << (m.cls & 0xff);
-    sc->h_lights = lights;
-#define UP(buf, vec)                                                                                     \
-    do {                                                                                                 \
-        cudaError_t e_ = sc->buf.upload(vec);                                                            \
-        if (e_ != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload " #buf ": ") + cudaGetErrorString(e_)); \
-        sc->upload_bytes += (vec).size() * sizeof((vec)[0]);                                             \
-    } while (0)
-    sc->upload_bytes += up_bytes;
-    since("nodes + triangles uploaded");
-    {   // wide records for the traversal (pb_trace.cuh): derived on the device from the node array that has just arrived
-        bool ok = desc->n_nodes > 1 && desc->nodes[0].n_prims == 0 && !any_alpha &&
-                  desc->n_nodes < (1u << PB_WIDE_LEAF_SHIFT) && desc->n_tris < (1u << PB_WIDE_LEAF_SHIFT) &&
-                  (desc->n_instances > 0 || (size_t)desc->n_nodes * 32 + (size_t)desc->n_tris * 48 > PB_TRACE_SMEM_BYTES) && max_leaf_prims.load() <= 15u;
-        if (ok) {
-            CK(sc->wide.alloc(4 * (size_t)desc->n_nodes));
-            k_wide_build<<<(desc->n_nodes + 255) / 256, 256>>>(sc->nodes.p, desc->n_nodes, sc->wide.p);
-            CK(cudaGetLastError());
-            g_launches++;
-        }
-    }
+        for (int k = 0; k < 5; ++k) P.halton[5 * s + k] = host_radical_inverse(k, (uint64_t)s);
+    // wide records for the traversal (pb_trace.cuh): derived on the device from the node array
+    P.wide = desc->n_nodes > 1 && desc->nodes[0].n_prims == 0 && !any_alpha &&
+             desc->n_nodes < (1u << PB_WIDE_LEAF_SHIFT) && desc->n_tris < (1u << PB_WIDE_LEAF_SHIFT) &&
+             (desc->n_instances > 0 || (size_t)desc->n_nodes * 32 + (size_t)desc->n_tris * 48 > PB_TRACE_SMEM_BYTES) && max_leaf_prims.load() <= 15u;
     // infinite lights: radiance map + Distribution2D tables (built on the host like InfiniteAreaLight::new does)
-    {
-        std::vector<DEnv> envs;
-        sc->h_env_power.assign(desc->n_lights, sp1(0.0f));
-        for (uint32_t k = 0; k < n_inf; ++k) {
-            const PbrtLight& l = desc->lights[inf_idx[k]];
-            HostEnv he;
-            build_env(l.env_texels, (int)l.env_res[0], (int)l.env_res[1], he);  // he.w / he.h: the power-of-two resolution after MipMap::new's resampling
-            sc->env_bufs.emplace_back(new PbrtScene::EnvBufs());
-            PbrtScene::EnvBufs& b = *sc->env_bufs.back();
-            cudaError_t e_ = b.texels.upload(he.texels);
-            if (e_ == cudaSuccess) e_ = b.cond_func.upload(he.cond_func);
-            if (e_ == cudaSuccess) e_ = b.cond_cdf.upload(he.cond_cdf);
-            if (e_ == cudaSuccess) e_ = b.cond_int.upload(he.cond_int);
-            if (e_ == cudaSuccess) e_ = b.marg_func.upload(he.marg_func);
-            if (e_ == cudaSuccess) e_ = b.marg_cdf.upload(he.marg_cdf);
-            if (e_ != cudaSuccess) { return fail(PBRT_E_CUDA, std::string("upload environment map: ") + cudaGetErrorString(e_)); }
-            sc->upload_bytes += he.texels.size() * 16 + (he.cond_func.size() + he.cond_cdf.size() + he.cond_int.size() + he.marg_func.size() + he.marg_cdf.size()) * 4;
-            DEnv de;
-            std::memset(&de, 0, sizeof de);
-            de.texels = b.texels.p; de.w = he.w; de.h = he.h; de.nu = he.nu; de.nv = he.nv;
-            de.cond_func = b.cond_func.p; de.cond_cdf = b.cond_cdf.p; de.cond_int = b.cond_int.p;
-            de.marg_func = b.marg_func.p; de.marg_cdf = b.marg_cdf.p; de.marg_int = he.marg_int;
-            std::memcpy(de.l2w, l.l2w, sizeof de.l2w);
-            std::memcpy(de.w2l, l.w2l, sizeof de.w2l);
-            lights[inf_idx[k]].env = (uint32_t)envs.size();
-            envs.push_back(de);
-            sc->h_env_power[inf_idx[k]] = he.power_L;
-        }
-        // goniometric and projection lights: MipMap::new (the Lanczos zoom and the pyramid) for level 0 and power()
-        for (uint32_t i = 0; i < desc->n_lights; ++i) {
-            const PbrtLight& l = desc->lights[i];
-            if (l.kind != PBRT_LIGHT_GONIOMETRIC && l.kind != PBRT_LIGHT_PROJECTION) continue;
-            DEnv de;
-            std::memset(&de, 0, sizeof de);
-            Sp lookup_half = sp1(1.0f);  // power(): Spectrum::new(1.0) without a map
-            if (l.env_texels) {
-                std::vector<MipLevel> pyr;
-                build_pyramid(l.env_texels, (int)l.env_res[0], (int)l.env_res[1], PBRT_WRAP_REPEAT, pyr);
-                std::vector<float4> t0((size_t)pyr[0].us * pyr[0].vs);
-                for (size_t q = 0; q < t0.size(); ++q) t0[q] = make_float4(pyr[0].t[q].r, pyr[0].t[q].g, pyr[0].t[q].b, 0.0f);
-                sc->env_bufs.emplace_back(new PbrtScene::EnvBufs());
-                cudaError_t e_ = sc->env_bufs.back()->texels.upload(t0);
-                if (e_ != cudaSuccess) { return fail(PBRT_E_CUDA, std::string("upload light map: ") + cudaGetErrorString(e_)); }
-                sc->upload_bytes += t0.size() * 16;
-                de.texels = sc->env_bufs.back()->texels.p; de.w = pyr[0].us; de.h = pyr[0].vs;
-                lookup_half = mip_lookup(pyr, 0.5f, 0.5f, 0.5f);
-            }
-            const Sp I = mksp(l.L[0], l.L[1], l.L[2]);
-            if (l.kind == PBRT_LIGHT_GONIOMETRIC) sc->h_env_power[i] = lookup_half * I * 4.0f * PB_PI;  // goniometric.rs:266-280
-            else {
-                projection_constants((float)l.env_res[0] / (float)l.env_res[1], l.fov, de.proj, de.screen, de.hither, lights[i].cos_total_width);
-                sc->h_env_power[i] = lookup_half * I * 2.0f * PB_PI * (1.0f - lights[i].cos_total_width);  // projection.rs:379-398
-            }
-            lights[i].env = (uint32_t)envs.size();
-            envs.push_back(de);
-        }
-        sc->h_lights = lights;
-        if (!envs.empty()) UP(envs, envs);
+    P.env_power.assign(desc->n_lights, sp1(0.0f));
+    for (uint32_t k = 0; k < n_inf; ++k) {
+        const PbrtLight& l = desc->lights[inf_idx[k]];
+        P.envs.emplace_back();
+        HostEnv& he = P.envs.back();
+        build_env(l.env_texels, (int)l.env_res[0], (int)l.env_res[1], he);  // he.w / he.h: the power-of-two resolution after MipMap::new's resampling
+        DEnv de;
+        std::memset(&de, 0, sizeof de);
+        de.w = he.w; de.h = he.h; de.nu = he.nu; de.nv = he.nv; de.marg_int = he.marg_int;
+        std::memcpy(de.l2w, l.l2w, sizeof de.l2w);
+        std::memcpy(de.w2l, l.w2l, sizeof de.w2l);
+        lights[inf_idx[k]].env = (uint32_t)P.denvs.size();
+        P.denvs.push_back(de);
+        P.env_power[inf_idx[k]] = he.power_L;
     }
-    if (!dinst.empty()) UP(instances, dinst);
+    // goniometric and projection lights: MipMap::new (the Lanczos zoom and the pyramid) for level 0 and power()
+    for (uint32_t i = 0; i < desc->n_lights; ++i) {
+        const PbrtLight& l = desc->lights[i];
+        if (l.kind != PBRT_LIGHT_GONIOMETRIC && l.kind != PBRT_LIGHT_PROJECTION) continue;
+        DEnv de;
+        std::memset(&de, 0, sizeof de);
+        P.envs.emplace_back();
+        Sp lookup_half = sp1(1.0f);  // power(): Spectrum::new(1.0) without a map
+        if (l.env_texels) {
+            std::vector<MipLevel> pyr;
+            build_pyramid(l.env_texels, (int)l.env_res[0], (int)l.env_res[1], PBRT_WRAP_REPEAT, pyr);
+            std::vector<float4>& t0 = P.envs.back().texels;
+            t0.resize((size_t)pyr[0].us * pyr[0].vs);
+            for (size_t q = 0; q < t0.size(); ++q) t0[q] = make_float4(pyr[0].t[q].r, pyr[0].t[q].g, pyr[0].t[q].b, 0.0f);
+            de.w = pyr[0].us; de.h = pyr[0].vs;
+            lookup_half = mip_lookup(pyr, 0.5f, 0.5f, 0.5f);
+        }
+        const Sp I = mksp(l.L[0], l.L[1], l.L[2]);
+        if (l.kind == PBRT_LIGHT_GONIOMETRIC) P.env_power[i] = lookup_half * I * 4.0f * PB_PI;  // goniometric.rs:266-280
+        else {
+            projection_constants((float)l.env_res[0] / (float)l.env_res[1], l.fov, de.proj, de.screen, de.hither, lights[i].cos_total_width);
+            P.env_power[i] = lookup_half * I * 2.0f * PB_PI * (1.0f - lights[i].cos_total_width);  // projection.rs:379-398
+        }
+        lights[i].env = (uint32_t)P.denvs.size();
+        P.denvs.push_back(de);
+    }
     if (any_alpha) {
-        std::vector<uint2> ma(desc->n_meshes);
-        for (uint32_t i = 0; i < desc->n_meshes; ++i) ma[i] = make_uint2(desc->meshes[i].alpha, desc->meshes[i].shadow_alpha);
-        UP(mesh_alpha, ma);
+        P.mesh_alpha.resize(desc->n_meshes);
+        for (uint32_t i = 0; i < desc->n_meshes; ++i) P.mesh_alpha[i] = make_uint2(desc->meshes[i].alpha, desc->meshes[i].shadow_alpha);
     }
+    P.tex_texels.resize(desc->n_textures);
     if (desc->n_textures) {  // ImageTexture::new -> MipMap::new on the host, the pyramid levels back to back on the device
-        std::vector<DTexture> dtex(desc->n_textures);
+        P.textures.resize(desc->n_textures);
         for (uint32_t i = 0; i < desc->n_textures; ++i) {
             const PbrtTexture& t = desc->textures[i];
             if (t.kind != PBRT_TEX_IMAGE) {  // constant / scale / mix: no pyramid
-                DTexture& dn = dtex[i];
+                DTexture& dn = P.textures[i];
                 std::memset(&dn, 0, sizeof dn);
                 dn.kind = t.kind;
                 dn.value[0] = t.value[0]; dn.value[1] = t.channels == 1 ? t.value[0] : t.value[1]; dn.value[2] = t.channels == 1 ? t.value[0] : t.value[2];
                 for (int c = 0; c < 3; ++c) dn.child[c] = t.child[c];
-                sc->tex_bufs.emplace_back(new DevBuf<float4>());
                 continue;
             }
             std::vector<MipLevel> pyr;
@@ -1298,48 +1241,56 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
             }
             build_pyramid(tex_rgb, (int)t.res[0], (int)t.res[1], t.wrap, pyr);
             if (pyr.size() > PB_MAX_MIP_LEVELS) { return fail(PBRT_E_UNSUPPORTED, "texture pyramid deeper than 16 levels"); }
-            DTexture& dt = dtex[i];
+            DTexture& dt = P.textures[i];
             std::memset(&dt, 0, sizeof dt);
-            std::vector<float4> flat;
+            std::vector<float4>& flat = P.tex_texels[i];
             for (size_t l = 0; l < pyr.size(); ++l) {
                 dt.off[l] = (uint32_t)flat.size();
                 for (const Sp& v : pyr[l].t) flat.push_back(make_float4(v.r, v.g, v.b, 0.0f));
             }
-            sc->tex_bufs.emplace_back(new DevBuf<float4>());
-            cudaError_t e_ = sc->tex_bufs.back()->upload(flat);
-            if (e_ != cudaSuccess) { return fail(PBRT_E_CUDA, std::string("upload texture: ") + cudaGetErrorString(e_)); }
-            sc->upload_bytes += flat.size() * 16;
-            dt.texels = sc->tex_bufs.back()->p;
             dt.w = pyr[0].us; dt.h = pyr[0].vs; dt.n_levels = (int)pyr.size();
             dt.wrap = t.wrap; dt.trilinear = t.trilinear ? 1u : 0u; dt.max_anisotropy = t.max_anisotropy;
             dt.su = t.su; dt.sv = t.sv; dt.du = t.du; dt.dv = t.dv;
             dt.mapping = t.mapping;
             std::memcpy(dt.map_m, t.map_m, sizeof dt.map_m);
         }
-        std::vector<float> lut(128);
+        P.ewa_lut.resize(128);
         for (int i = 0; i < 128; ++i) {  // mipmap.rs:188-195
             const float alpha = 2.0f, r2 = (float)i / (float)(128 - 1);
-            lut[i] = expf(-alpha * r2) - expf(-alpha);
+            P.ewa_lut[i] = expf(-alpha * r2) - expf(-alpha);
         }
-        UP(textures, dtex); UP(mat_src, mat_src); UP(ewa_lut, lut);
     }
     for (uint32_t i = 0; i < desc->n_materials; ++i) mats_single[i].cls = mats[i].cls;
-    UP(materials_single, mats_single);
-    UP(materials, mats); UP(lights, lights); UP(m32, m32); UP(nib, nib); UP(vdc, vdc); UP(vdci, vdci); UP(halton, halton);
-#undef UP
-    DScene& d = sc->d;
+    for (const DLight& l : lights) P.light_level = std::max(P.light_level, l.kind == PBRT_LIGHT_DIFFUSE_AREA ? 0 : l.kind < PBRT_LIGHT_GONIOMETRIC ? 1 : 2);
+    for (const DMaterial& m : mats) P.class_mask |= 1u << (m.cls & 0xff);
+    // ---- the large arrays, as the device holds them: the caller's nodes, triangle records and per-vertex attributes (concatenated over
+    // the meshes), then the texture pyramids
+    P.big.resize(BIG_TEX0 + desc->n_textures);
+    auto whole = [&](int a, const void* src, size_t bytes, size_t elem) { P.big[a].bytes = bytes; P.big[a].elem = elem; if (bytes) P.big[a].pieces.push_back({0, src, bytes}); };
+    whole(BIG_TRIS, desc->tris, 24 * (size_t)desc->n_tris, 24);
+    whole(BIG_NODES, desc->nodes, 32 * (size_t)desc->n_nodes, 32);
+    for (uint32_t i = 0; i < desc->n_textures; ++i) whole(BIG_TEX0 + i, P.tex_texels[i].data(), 16 * P.tex_texels[i].size(), 16);
+    const struct { int a; bool any; size_t width; } attrs[] = {{BIG_P, true, 12}, {BIG_N, any_n, 12}, {BIG_UV, any_uv, 8}, {BIG_S, any_s, 12}};
+    for (const auto& at : attrs) {
+        if (!at.any) continue;
+        P.big[at.a].bytes = at.width * total_verts;
+        P.big[at.a].elem = at.width;
+        for (uint32_t i = 0; i < desc->n_meshes; ++i) {
+            const PbrtMesh& m = desc->meshes[i];
+            const float* src = at.a == BIG_P ? m.p : at.a == BIG_N ? m.n : at.a == BIG_UV ? m.uv : m.s;
+            if (src && m.n_verts) P.big[at.a].pieces.push_back({at.width * vbase[i], src, at.width * (size_t)m.n_verts});
+        }
+    }
+    // ---- the scene record without its device pointers
+    DScene& d = P.d;
     std::memset(&d, 0, sizeof d);
-    d.nodes = sc->nodes.p; d.n_nodes = desc->n_nodes;
-    d.wide = sc->wide.p;
-    d.tri_verts = sc->tri_verts.p; d.n_tris = desc->n_tris;
-    d.tri_idx = sc->tri_idx.p;
-    d.vn = sc->vn.p; d.vuv = sc->vuv.p; d.vs = sc->vs.p;
-    d.materials = sc->materials.p; d.n_materials = desc->n_materials;
-    d.lights = sc->lights.p; d.n_lights = desc->n_lights;
-    d.envs = sc->envs.p; d.n_inf = n_inf;
-    d.instances = sc->instances.p; d.n_instances = desc->n_instances;
-    d.mesh_alpha = sc->mesh_alpha.p;
-    d.textures = sc->textures.p; d.mat_src = sc->mat_src.p; d.ewa_lut = sc->ewa_lut.p; d.n_textures = desc->n_textures;
+    d.n_nodes = desc->n_nodes;
+    d.n_tris = desc->n_tris;
+    d.n_materials = desc->n_materials;
+    d.n_lights = desc->n_lights;
+    d.n_inf = n_inf;
+    d.n_instances = desc->n_instances;
+    d.n_textures = desc->n_textures;
     {  // dx_camera / dy_camera, PerspectiveCamera::new (perspective.rs:82-99)
         auto r2c = [&](float x, float y) {
             const float* m = desc->camera.raster_to_camera;
@@ -1364,64 +1315,332 @@ int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out
         bool inside = c.x >= pmin.x && c.x <= pmax.x && c.y >= pmin.y && c.y <= pmax.y && c.z >= pmin.z && c.z <= pmax.z;
         d.world_radius = inside ? len3(c - pmax) : 0.0f;
     }
+    return PBRT_OK;
+}
+
+// One device's part of a scene_create call: the replica under construction and the temporaries its flattening reads, which the
+// other devices may still be copying from until every device is done.
+struct SceneBuild {
+    static constexpr size_t slot_bytes = (size_t)64 << 20;
+    int device = 0;
+    uint32_t part = 0, n_parts = 1;
+    DeviceScratch* scr = nullptr;
+    std::unique_ptr<PbrtScene> sc;
+    DevBuf<uint2> raw_tris;   // the caller's PbrtTri records as they are (24 B each), flattened on the device
+    DevBuf<float> raw_p;      // mesh positions, concatenated
+    DevBuf<DMeshRec> d_meshes;
+    DevBuf<uint32_t> d_status;
+    std::vector<unsigned char*> dst;  // where each BigArray lives on this device
+    bool slot_used[2] = {false, false};
+    int next_slot = 0;
+    unsigned copy_threads = 1;
+    size_t up_bytes = 0;  // host -> device bytes of this replica
+    void release() {
+        sc.reset();
+        raw_tris.release(); raw_p.release(); d_meshes.release(); d_status.release();
+    }
+    // A source array in pinned memory (the caller's own cudaHostAlloc / pbrt_gpu_host_register) is DMA'd where it lies; pageable
+    // memory goes through two pinned staging slots, copied into them on several cores while the previous slot is in flight (a
+    // cudaMemcpy straight from pageable memory runs at a fraction of the pinned rate).
+    cudaError_t upload(void* to, const void* src, size_t bytes) {
+        if (!bytes) return cudaSuccess;
+        up_bytes += bytes;
+        cudaStream_t ups = scr->up_stream[1];
+        cudaPointerAttributes at;
+        const bool pinned = cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost;
+        cudaGetLastError();
+        if (pinned) return cudaMemcpyAsync(to, src, bytes, cudaMemcpyHostToDevice, ups);
+        for (size_t off = 0; off < bytes; off += slot_bytes) {
+            const size_t n = std::min(slot_bytes, bytes - off);
+            const int k = next_slot;
+            next_slot ^= 1;
+            if (slot_used[k]) { cudaError_t e = cudaEventSynchronize(scr->slot_ev[k]); if (e != cudaSuccess) return e; }
+            unsigned char* stage = scr->stage + (size_t)k * slot_bytes;
+            const unsigned char* from = static_cast<const unsigned char*>(src) + off;
+            if (n < ((size_t)1 << 20) || copy_threads == 1) std::memcpy(stage, from, n);
+            else {
+                const unsigned nt = copy_threads;
+                std::vector<std::thread> th;
+                for (unsigned t = 0; t < nt; ++t) th.emplace_back([=] { const size_t lo = n * t / nt, hi = n * (t + 1) / nt; std::memcpy(stage + lo, from + lo, hi - lo); });
+                for (auto& x : th) x.join();
+            }
+            cudaError_t e = cudaMemcpyAsync(static_cast<unsigned char*>(to) + off, stage, n, cudaMemcpyHostToDevice, ups);
+            if (e == cudaSuccess) e = cudaEventRecord(scr->slot_ev[k], ups);
+            if (e != cudaSuccess) return e;
+            slot_used[k] = true;
+        }
+        return cudaSuccess;
+    }
+    // bytes [lo, hi) of array a from the host
+    cudaError_t upload_range(const BigArray& a, unsigned char* to, size_t lo, size_t hi) {
+        for (const BigArray::Piece& p : a.pieces) {
+            const size_t s = std::max(lo, p.off), e = std::min(hi, p.off + p.bytes);
+            if (s >= e) continue;
+            cudaError_t rc = upload(to + s, static_cast<const unsigned char*>(p.src) + (s - p.off), e - s);
+            if (rc != cudaSuccess) return rc;
+        }
+        return cudaSuccess;
+    }
+};
+
+// Allocates the replica and uploads this device's slice of every large array; shard_ev marks the slices as arrived.
+static int build_begin(const ScenePrep& P, SceneBuild& b) {
+    const PbrtSceneDesc* desc = P.desc;
+    CK(cudaSetDevice(b.device));
+    b.sc.reset(new PbrtScene());
+    PbrtScene* sc = b.sc.get();
+    sc->device = b.device;
+    sc->recycle_buffers(b.device);
+    b.raw_tris.cache_dev = b.raw_p.cache_dev = b.d_meshes.cache_dev = b.d_status.cache_dev = b.device;
+    CK(sc->nodes.alloc(2 * (size_t)desc->n_nodes));
+    CK(sc->tri_verts.alloc(3 * (size_t)desc->n_tris));
+    CK(sc->tri_idx.alloc((size_t)desc->n_tris));
+    CK(b.raw_tris.alloc(3 * (size_t)desc->n_tris));
+    CK(b.raw_p.alloc(3 * P.total_verts));
+    if (P.any_n) CK(sc->vn.alloc(3 * P.total_verts));
+    if (P.any_uv) CK(sc->vuv.alloc(2 * P.total_verts));
+    if (P.any_s) CK(sc->vs.alloc(3 * P.total_verts));
+    CK(b.d_meshes.alloc(P.meshes.size()));
+    CK(b.d_status.alloc(2));
+    for (const std::vector<float4>& t : P.tex_texels) {
+        sc->tex_bufs.emplace_back(new DevBuf<float4>());
+        CK(sc->tex_bufs.back()->alloc(t.size()));
+    }
+    b.dst = {reinterpret_cast<unsigned char*>(b.raw_tris.p), reinterpret_cast<unsigned char*>(b.raw_p.p), reinterpret_cast<unsigned char*>(sc->nodes.p),
+             reinterpret_cast<unsigned char*>(sc->vn.p), reinterpret_cast<unsigned char*>(sc->vuv.p), reinterpret_cast<unsigned char*>(sc->vs.p)};
+    for (const auto& t : sc->tex_bufs) b.dst.push_back(reinterpret_cast<unsigned char*>(t->p));
+    CK(b.scr->staging(2 * SceneBuild::slot_bytes));
+    cudaStream_t ups = b.scr->up_stream[1];
+    cudaError_t e = cudaMemcpyAsync(b.d_meshes.p, P.meshes.data(), P.meshes.size() * sizeof(DMeshRec), cudaMemcpyHostToDevice, ups);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b.d_status.p, 0, 8, ups);
+    for (size_t a = 0; a < P.big.size() && e == cudaSuccess; ++a) {
+        size_t lo, hi;
+        P.big[a].slice(b.part, b.n_parts, lo, hi);
+        e = b.upload_range(P.big[a], b.dst[a], lo, hi);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(b.scr->shard_ev, ups);
+    if (e != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload scene arrays: ") + cudaGetErrorString(e));
+    return PBRT_OK;
+}
+
+// Completes the large arrays of replica i -- the other slices from the devices that uploaded them, or from the host where a pair has
+// no peer access --, flattens the triangles, and uploads the small host-made tables.
+static int build_finish(const ScenePrep& P, std::vector<SceneBuild>& builds, uint32_t i) {
+    const PbrtSceneDesc* desc = P.desc;
+    SceneBuild& b = builds[i];
+    PbrtScene* sc = b.sc.get();
+    CK(cudaSetDevice(b.device));
+    cudaStream_t ups = b.scr->up_stream[1];
+    std::vector<bool> peer(builds.size(), false);
+    for (uint32_t j = 0; j < builds.size(); ++j) {
+        if (j == i || !enable_peer_access(b.device, builds[j].device)) continue;
+        peer[j] = true;
+        CK(cudaStreamWaitEvent(ups, builds[j].scr->shard_ev, 0));
+    }
+    auto complete = [&](size_t a) -> cudaError_t {
+        for (uint32_t j = 0; j < builds.size(); ++j) {
+            if (j == i) continue;
+            size_t lo, hi;
+            P.big[a].slice(builds[j].part, b.n_parts, lo, hi);
+            if (lo == hi) continue;
+            cudaError_t e = peer[j] ? cudaMemcpyPeerAsync(b.dst[a] + lo, b.device, builds[j].dst[a] + lo, builds[j].device, hi - lo, ups)
+                                    : b.upload_range(P.big[a], b.dst[a], lo, hi);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    };
+    cudaError_t e = complete(BIG_TRIS);
+    if (e == cudaSuccess) e = complete(BIG_P);
+    if (e != cudaSuccess) return fail(PBRT_E_CUDA, std::string("complete triangles / positions: ") + cudaGetErrorString(e));
+    // triangles: validated and pre-gathered (vertices in BVH order) on the device
+    if (desc->n_tris) {
+        k_flatten_tris<<<(desc->n_tris + 255) / 256, 256, 0, ups>>>(b.raw_tris.p, desc->n_tris, b.d_meshes.p, desc->n_meshes, b.raw_p.p, desc->n_materials, desc->n_lights,
+                                                                   desc->n_instances, sc->tri_verts.p, sc->tri_idx.p, b.d_status.p);
+        g_launches++;
+    }
+    for (size_t a = BIG_NODES; a < P.big.size() && e == cudaSuccess; ++a) e = complete(a);
+    if (e != cudaSuccess) return fail(PBRT_E_CUDA, std::string("complete nodes / vertex attributes / textures: ") + cudaGetErrorString(e));
+    uint32_t h_status[2] = {0, 0};
+    CK(cudaMemcpyAsync(h_status, b.d_status.p, 8, cudaMemcpyDeviceToHost, ups));
+    CK(cudaStreamSynchronize(ups));  // (the staging slots and the temporaries are quiet from here on)
+    CK(cudaGetLastError());
+    if (h_status[0]) return tri_fail((int)h_status[0]);
+    sc->has_null_material = h_status[1] != 0;
+    sc->h_nib = P.nib;
+    sc->light_level = P.light_level;
+    sc->class_mask = P.class_mask;
+    sc->h_lights = P.lights;
+    sc->h_env_power = P.env_power;
+    sc->upload_bytes = b.up_bytes;
+#define UP(buf, vec)                                                                                     \
+    do {                                                                                                 \
+        cudaError_t e_ = sc->buf.upload(vec);                                                            \
+        if (e_ != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload " #buf ": ") + cudaGetErrorString(e_)); \
+        sc->upload_bytes += (vec).size() * sizeof((vec)[0]);                                             \
+    } while (0)
+    if (P.wide) {  // wide records for the traversal (pb_trace.cuh): derived on the device from the node array that has just arrived
+        CK(sc->wide.alloc(4 * (size_t)desc->n_nodes));
+        k_wide_build<<<(desc->n_nodes + 255) / 256, 256>>>(sc->nodes.p, desc->n_nodes, sc->wide.p);
+        CK(cudaGetLastError());
+        g_launches++;
+    }
+    std::vector<DEnv> envs = P.denvs;
+    for (size_t k = 0; k < P.envs.size(); ++k) {
+        const HostEnv& he = P.envs[k];
+        sc->env_bufs.emplace_back(new PbrtScene::EnvBufs());
+        PbrtScene::EnvBufs& eb = *sc->env_bufs.back();
+        cudaError_t e_ = eb.texels.upload(he.texels);
+        if (e_ == cudaSuccess) e_ = eb.cond_func.upload(he.cond_func);
+        if (e_ == cudaSuccess) e_ = eb.cond_cdf.upload(he.cond_cdf);
+        if (e_ == cudaSuccess) e_ = eb.cond_int.upload(he.cond_int);
+        if (e_ == cudaSuccess) e_ = eb.marg_func.upload(he.marg_func);
+        if (e_ == cudaSuccess) e_ = eb.marg_cdf.upload(he.marg_cdf);
+        if (e_ != cudaSuccess) return fail(PBRT_E_CUDA, std::string("upload environment / light map: ") + cudaGetErrorString(e_));
+        sc->upload_bytes += he.texels.size() * 16 + (he.cond_func.size() + he.cond_cdf.size() + he.cond_int.size() + he.marg_func.size() + he.marg_cdf.size()) * 4;
+        DEnv& de = envs[k];
+        de.texels = eb.texels.p;
+        if (k < P.d.n_inf) {  // (a light map keeps its projection constants in the same union)
+            de.cond_func = eb.cond_func.p; de.cond_cdf = eb.cond_cdf.p; de.cond_int = eb.cond_int.p;
+            de.marg_func = eb.marg_func.p; de.marg_cdf = eb.marg_cdf.p;
+        }
+    }
+    if (!envs.empty()) UP(envs, envs);
+    if (!P.instances.empty()) UP(instances, P.instances);
+    if (P.any_alpha) UP(mesh_alpha, P.mesh_alpha);
+    if (desc->n_textures) {
+        std::vector<DTexture> dtex = P.textures;
+        for (uint32_t t = 0; t < desc->n_textures; ++t) if (desc->textures[t].kind == PBRT_TEX_IMAGE) dtex[t].texels = sc->tex_bufs[t]->p;
+        UP(textures, dtex); UP(mat_src, P.mat_src); UP(ewa_lut, P.ewa_lut);
+    }
+    UP(materials_single, P.mats_single);
+    UP(materials, P.mats); UP(lights, P.lights); UP(m32, P.m32); UP(nib, P.nib); UP(vdc, P.vdc); UP(vdci, P.vdci); UP(halton, P.halton);
+#undef UP
+    DScene& d = sc->d;
+    d = P.d;
+    d.nodes = sc->nodes.p;
+    d.wide = sc->wide.p;
+    d.tri_verts = sc->tri_verts.p;
+    d.tri_idx = sc->tri_idx.p;
+    d.vn = sc->vn.p; d.vuv = sc->vuv.p; d.vs = sc->vs.p;
+    d.materials = sc->materials.p;
+    d.lights = sc->lights.p;
+    d.envs = sc->envs.p;
+    d.instances = sc->instances.p;
+    d.mesh_alpha = sc->mesh_alpha.p;
+    d.textures = sc->textures.p; d.mat_src = sc->mat_src.p; d.ewa_lut = sc->ewa_lut.p;
+    // a camera whose keyframes are equal takes the static kernels: interpolate() would hand back the start transform at every time
+    sc->cam_motion = P.cam_mo.actually_animated != 0;
+    sc->cam_mo = P.cam_mo;
     CK(cudaDeviceSynchronize());
-    stage_lock.unlock();
-    *out = sc_guard.release();
+    return PBRT_OK;
+}
+
+// The scene on devices[0..n) (distinct, already checked by the caller): out[k] is the replica on devices[k], or every out[k] is null.
+static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n, PbrtScene** out) {
+    static const int timing = getenv("PB_TIMING") ? atoi(getenv("PB_TIMING")) : 0;  // 1: every call; 2: only calls slower than 100 ms
+    const auto t_enter = std::chrono::steady_clock::now();
+    std::string timing_log;
+    auto since = [&](const char* what) {
+        if (!timing) return;
+        char line[160];
+        snprintf(line, sizeof line, "[pb timing] scene_create %-26s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enter).count());
+        if (timing == 1) fputs(line, stderr); else timing_log += line;
+    };
+    struct SlowDump { std::string& log; const std::chrono::steady_clock::time_point t0; int mode; ~SlowDump() {
+        if (mode == 2 && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() > 100.0) fputs(log.c_str(), stderr); } } slow_dump{timing_log, t_enter, timing};
+    for (uint32_t k = 0; k < n; ++k) out[k] = nullptr;
+    ScenePrep P;
+    int rc = scene_prepare(desc, motion, P);
+    if (rc != PBRT_OK) return rc;
+    since("host preparation");
+    for (uint32_t k = 0; k < n; ++k) {
+        rc = check_device(devices[k]);
+        if (rc != PBRT_OK) {
+            // no usable device: a malformed description is still reported as such (validation does not depend on the hardware; it is
+            // otherwise fused with the flattening on the device)
+            const std::string dev_err = g_err;
+            const int vrc = parallel_for(desc->n_tris, [&](uint32_t lo, uint32_t hi) -> int {
+                for (uint32_t i = lo; i < hi; ++i) if (int e = tri_error(desc, desc->tris[i])) return e;
+                return 0;
+            });
+            if (vrc) return tri_fail(vrc);
+            return fail(rc, dev_err);
+        }
+    }
+    // scene creation is serialised per device (the pinned staging and the upload streams are the device's); the locks are taken in
+    // device order, so that two calls over overlapping device sets cannot deadlock
+    std::vector<SceneBuild> builds(n);
+    std::vector<uint32_t> order(n);
+    for (uint32_t k = 0; k < n; ++k) order[k] = k;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t c) { return devices[a] < devices[c]; });
+    std::vector<std::unique_lock<std::mutex>> locks;
+    const unsigned copy_threads = std::max(1u, host_threads() / n);
+    for (uint32_t k : order) {
+        SceneBuild& b = builds[k];
+        b.device = devices[k]; b.part = k; b.n_parts = n; b.copy_threads = copy_threads;
+        if (!(b.scr = scratch_for(b.device))) return fail(PBRT_E_INVALID, "device ordinal out of range");
+        locks.emplace_back(b.scr->stage_mu);
+        CK(cudaSetDevice(b.device));
+        if (!b.scr->pool_ready) {
+            for (int s = 0; s < 2; ++s) CK(cudaStreamCreateWithFlags(&b.scr->up_stream[s], cudaStreamNonBlocking));
+            for (int s = 0; s < 2; ++s) CK(cudaEventCreateWithFlags(&b.scr->slot_ev[s], cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&b.scr->shard_ev, cudaEventDisableTiming));
+            b.scr->pool_ready = true;
+        }
+    }
+    // one host thread per device; every device's own slices are queued before any device starts copying from its peers
+    std::vector<int> rcs(n, PBRT_OK);
+    std::vector<std::string> errs(n);
+    auto run = [&](const std::function<int(uint32_t)>& step) -> int {
+        auto one = [&](uint32_t k) { rcs[k] = step(k); if (rcs[k] != PBRT_OK) errs[k] = g_err; };
+        if (n == 1) one(0);
+        else {
+            std::vector<std::thread> th;
+            for (uint32_t k = 0; k < n; ++k) th.emplace_back(one, k);
+            for (auto& t : th) t.join();
+        }
+        for (uint32_t k = 0; k < n; ++k)
+            if (rcs[k] != PBRT_OK) return fail(rcs[k], (n > 1 && rcs[k] == PBRT_E_CUDA ? "device " + std::to_string(devices[k]) + ": " : std::string()) + errs[k]);
+        return PBRT_OK;
+    };
+    rc = run([&](uint32_t k) { return build_begin(P, builds[k]); });
+    since("own slices queued");
+    if (rc == PBRT_OK) rc = run([&](uint32_t k) { return build_finish(P, builds, k); });
+    since("replicas complete");
+    if (rc != PBRT_OK) {
+        // nothing goes back to a BufCache while a device may still write it or read it for a peer
+        const std::string err = g_err;
+        for (SceneBuild& b : builds) if (cudaSetDevice(b.device) == cudaSuccess) cudaDeviceSynchronize();
+        for (SceneBuild& b : builds) { cudaSetDevice(b.device); b.release(); }
+        g_err = err;
+        return rc;
+    }
+    for (uint32_t k = 0; k < n; ++k) out[k] = builds[k].sc.release();
+    cudaSetDevice(devices[0]);
     since("done");
     return PBRT_OK;
 }
 
-static bool finite_keyframes(const PbrtAnimatedTransform& a) {
-    bool ok = std::isfinite(a.start_time) && std::isfinite(a.end_time);
-    for (int k = 0; k < 16; ++k)
-        ok = ok && std::isfinite(a.start[k]) && std::isfinite(a.start_inv[k]) && std::isfinite(a.end[k]) && std::isfinite(a.end_inv[k]);
-    return ok;
-}
+extern "C" {
 
-// m_inv is the inverse of m up to f32 rounding: every element of m * m_inv (in f64) lies within 1e-4 of the sum of the magnitudes of
-// its terms of the identity's element.  A caller that hands over another matrix's inverse (or a transposed one) is caught here.
-static bool inverse_pair(const float* m, const float* m_inv) {
-    for (int i = 0; i < 4; ++i)
-        for (int j = 0; j < 4; ++j) {
-            double p = 0.0, mag = 0.0;
-            for (int k = 0; k < 4; ++k) { p += (double)m[4 * i + k] * m_inv[4 * k + j]; mag += std::fabs((double)m[4 * i + k] * m_inv[4 * k + j]); }
-            if (!(std::fabs(p - (i == j ? 1.0 : 0.0)) <= 1e-4 * mag + 1e-6)) return false;
-        }
-    return true;
+int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out) {
+    if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
+    return create_scenes(desc, nullptr, &device, 1, out);
 }
 
 int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out) {
-    if (!motion) return pbrt_gpu_scene_create(desc, device, out);
     if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    *out = nullptr;
-    if (motion->instances) {
-        if (desc->n_instances && !desc->instances) return fail(PBRT_E_INVALID, "null instance array in scene description");
-        for (uint32_t i = 0; i < desc->n_instances; ++i) {
-            const PbrtAnimatedTransform& a = motion->instances[i];
-            if (!finite_keyframes(a)) return fail(PBRT_E_UNSUPPORTED, "instance keyframe matrix or time is not finite");
-            if (std::memcmp(a.start, desc->instances[i].m, 64) != 0 || std::memcmp(a.start_inv, desc->instances[i].m_inv, 64) != 0)
-                return fail(PBRT_E_INVALID, "an instance's start keyframe differs from PbrtInstance.m / m_inv");
-            for (int k = 0; k < 16; ++k)
-                if (a.start[k] != a.end[k] || a.start_inv[k] != a.end_inv[k])
-                    return fail(PBRT_E_UNSUPPORTED, "animated object instances are outside the GPU path");
-        }
-    }
-    DMotion cam_mo;
-    std::memset(&cam_mo, 0, sizeof cam_mo);
-    if (const PbrtAnimatedTransform* c = motion->camera) {
-        if (!finite_keyframes(*c)) return fail(PBRT_E_UNSUPPORTED, "camera keyframe matrix or time is not finite");
-        if (std::memcmp(c->start, desc->camera.camera_to_world, 64) != 0)
-            return fail(PBRT_E_INVALID, "the camera's start keyframe differs from PbrtCamera.camera_to_world");
-        if (!inverse_pair(c->start, c->start_inv) || !inverse_pair(c->end, c->end_inv))
-            return fail(PBRT_E_INVALID, "a camera keyframe's m_inv is not the inverse of its m");
-        motion_create(c->start, c->start_inv, c->start_time, c->end, c->end_inv, c->end_time, cam_mo);
-    }
-    const int rc = pbrt_gpu_scene_create(desc, device, out);
-    if (rc != PBRT_OK) return rc;
-    // a camera whose keyframes are equal takes the static kernels: interpolate() would hand back the start transform at every time
-    (*out)->cam_motion = cam_mo.actually_animated != 0;
-    (*out)->cam_mo = cam_mo;
-    return PBRT_OK;
+    return create_scenes(desc, motion, &device, 1, out);
+}
+
+int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n_devices, PbrtScene** out) {
+    if (!desc || !devices || !out || n_devices == 0) return fail(PBRT_E_INVALID, "null argument or no device");
+    for (uint32_t k = 0; k < n_devices; ++k) out[k] = nullptr;
+    if (n_devices > 16) return fail(PBRT_E_UNSUPPORTED, "more than 16 devices");
+    for (uint32_t k = 0; k < n_devices; ++k)
+        for (uint32_t j = 0; j < k; ++j)
+            if (devices[j] == devices[k]) return fail(PBRT_E_INVALID, "a device is listed twice (one replica per device)");
+    return create_scenes(desc, motion, devices, n_devices, out);
 }
 
 int pbrt_gpu_host_register(const void* ptr, uint64_t bytes) {
@@ -2447,14 +2666,7 @@ int pbrt_gpu_render_multi(PbrtScene* const* scenes, uint32_t n_scenes, const Pbr
     direct.n = 0;
     DevBuf<float> staged;
     for (uint32_t i = 1; i < n_scenes && npx; ++i) {
-        int can = 0;
-        CK(cudaDeviceCanAccessPeer(&can, root, scenes[i]->device));
-        if (can) {
-            cudaError_t e = cudaDeviceEnablePeerAccess(scenes[i]->device, 0);
-            if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); e = cudaSuccess; }
-            if (e != cudaSuccess) can = 0;
-        }
-        if (can) direct.p[direct.n++] = reinterpret_cast<const float4*>(scr[i]->film.p);
+        if (enable_peer_access(root, scenes[i]->device)) direct.p[direct.n++] = reinterpret_cast<const float4*>(scr[i]->film.p);
         else {
             CK(staged.alloc(npx * 4));
             CK(cudaMemcpyPeerAsync(staged.p, root, scr[i]->film.p, scenes[i]->device, npx * 16, 0));

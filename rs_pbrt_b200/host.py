@@ -456,6 +456,25 @@ def unpin_description(handle):
         L.pbrt_gpu_host_unregister(C.c_void_p(a))
 
 
+def create_multi(desc, devices, motion=None, lib=None):
+    """pbrt_gpu_scene_create_multi: the scene on every device of `devices` in one call, each large array crossing PCIe once; returns one
+    GpuScene per device, in the order given.  `motion`: as for GpuScene."""
+    L = lib if lib is not None else _abi.load()
+    devs = (C.c_int * len(devices))(*[int(d) for d in devices])
+    handles = (C.c_void_p * max(len(devices), 1))()
+    if motion is not None and not isinstance(motion, C._Pointer):
+        motion = C.pointer(motion)
+    rc = L.pbrt_gpu_scene_create_multi(desc, motion, devs, len(devices), handles)
+    if rc != 0:
+        raise PbrtError(rc, L.pbrt_gpu_last_error().decode())
+    out = []
+    for h in handles[: len(devices)]:
+        g = GpuScene.__new__(GpuScene)
+        g.L, g.handle = L, C.c_void_p(h)
+        out.append(g)
+    return out
+
+
 def render_multi(gpu_scenes, params, film=None):
     """pbrt_gpu_render_multi: one frame on several devices from this process (one GpuScene per device), into a host film."""
     L = gpu_scenes[0].L
