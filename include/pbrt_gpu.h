@@ -23,7 +23,8 @@
  * whitted integrators (PbrtRenderParams.direct_strategy); 4 = PbrtStats.shade_slots / shaded_vertices, tile-interleaved rendering
  * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi); within 4, the animated camera
  * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed); within 4, goniometric and projection lights
- * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word); within 4, pbrt_gpu_scene_create_multi.  Structs only ever grow at their end
+ * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word); within 4, pbrt_gpu_scene_create_multi; within 4,
+ * orthographic and environment cameras (pbrt_gpu_scene_create_camera, PbrtCameraModel).  Structs only ever grow at their end
  * within a version step, and a zero-initialised new field means "as before".
  */
 #ifndef PBRT_GPU_H
@@ -381,6 +382,37 @@ int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc
  * PBRT_E_UNSUPPORTED; a bad description or device: what pbrt_gpu_scene_create returns.  On any error every out[i] is NULL. */
 int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n_devices,
                                 PbrtScene** out);
+
+/* ---- camera models (ABI v4) ----------------------------------------------------------------------------------------------------
+ * PbrtCamera describes a PerspectiveCamera; a PbrtCameraModel handed to pbrt_gpu_scene_create_camera selects another of rs_pbrt's
+ * cameras (api.rs:1639-1689).  Every kind draws the same CameraSample (p_film, time, p_lens), traces at ray.time = lerp(sample.time,
+ * shutter_open, shutter_close) and goes through camera_to_world, animated or not (PbrtMotionDesc.camera).  What each kind reads:
+ *   PERSPECTIVE   PerspectiveCamera (src/cameras/perspective.rs:190-280): every field of PbrtCamera.  The model's other fields are
+ *                 ignored.
+ *   ORTHOGRAPHIC  OrthographicCamera (src/cameras/orthographic.rs:38-235): raster_to_camera (the caller builds it from
+ *                 Transform::orthographic(0, 1), the screen window and the FULL film resolution, :47-74), camera_to_world,
+ *                 lens_radius, focal_distance, the shutter.  The ray starts at raster_to_camera(p_film) along +z.  dx_camera /
+ *                 dy_camera are raster_to_camera.transform_vector of the unit raster steps (:75-84).  Without a lens the
+ *                 differentials are the origin shifted by dx_camera / dy_camera with the ray's direction.  With a lens both
+ *                 differentials aim at ONE focus point, p_camera + dx_camera + (0,0,1) * (focal_distance / d.z) of the already
+ *                 refracted d (:181-212): ry equals rx, and dy_camera is never used.
+ *   ENVIRONMENT   EnvironmentCamera (src/cameras/environment.rs:92-116): camera_to_world and the shutter only.  theta = pi * p_film.y /
+ *                 full_resolution[1], phi = 2 pi * p_film.x / full_resolution[0], d = (sin theta cos phi, cos theta, sin theta sin
+ *                 phi) from the origin.  The ray has NO differential (differential: None), so the first hit's texture lookups are
+ *                 level-0 lookups, like a later bounce's.  raster_to_camera and the lens are not read.
+ * full_resolution is Film.full_resolution {x, y}: the environment camera divides by it; the crop window does not change it.
+ * An unknown kind (RealisticCamera included) is PBRT_E_UNSUPPORTED; an ENVIRONMENT model with a zero full_resolution is
+ * PBRT_E_INVALID. */
+typedef enum PbrtCameraKind { PBRT_CAMERA_PERSPECTIVE = 0, PBRT_CAMERA_ORTHOGRAPHIC = 1, PBRT_CAMERA_ENVIRONMENT = 2 } PbrtCameraKind;
+typedef struct PbrtCameraModel {
+    uint32_t kind;               /* PbrtCameraKind */
+    uint32_t full_resolution[2]; /* ENVIRONMENT: Film.full_resolution {x, y} */
+} PbrtCameraModel;
+/* pbrt_gpu_scene_create_multi with a camera model; camera == NULL is the perspective camera, motion may be NULL, and n_devices == 1
+ * is a single scene.  pbrt_gpu_scene_create, _create_motion and _create_multi are this call with camera == NULL.  Errors as for
+ * pbrt_gpu_scene_create_multi, and those of the camera model above. */
+int pbrt_gpu_scene_create_camera(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices,
+                                 uint32_t n_devices, PbrtScene** out);
 void pbrt_gpu_scene_destroy(PbrtScene* scene);
 /* Optional (ABI v4): page-lock a host array the caller owns -- nodes, tris, a mesh's p / n / s / uv -- so that pbrt_gpu_scene_create
  * DMAs it where it lies (cudaHostRegister, portable across devices); an array that is not pinned is copied through the library's

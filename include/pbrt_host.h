@@ -4,7 +4,8 @@
  * rs_pbrt is compiled Rust and this image has no Rust toolchain, so the host side of the drop-in is
  * written in C++ and mirrors the reference's own call sequence for the path:
  *   pbrt_shape / pbrt_area_light_source      src/core/api.rs:2792-2870   -> pbrt_host_add_trianglemesh
- *   pbrt_look_at / make_camera               src/core/api.rs:486-514, src/cameras/perspective.rs:46-185
+ *   pbrt_look_at / make_camera               src/core/api.rs:486-514,1639-1689, src/cameras/perspective.rs:46-185,
+ *                                            orthographic.rs:99-149, environment.rs:44-90
  *   pbrt_transform_times / animated camera   src/core/api.rs:497-502,2525-2529 -> pbrt_host_camera_motion
  *   make_film / make_filter                  src/core/film.rs:176-262, src/filters
  *   make_sampler ("sobol")                   src/samplers/sobol.rs:37-108
@@ -102,6 +103,14 @@ int pbrt_host_film(PbrtHost* h, int xres, int yres, const float* crop, const cha
 /* Camera "perspective"; screen_window = {xmin,xmax,ymin,ymax} or NULL (derived from the frame aspect ratio). Call after pbrt_host_film. */
 int pbrt_host_camera_perspective(PbrtHost* h, float fov, float lens_radius, float focal_distance, float shutter_open, float shutter_close,
                                  const float* screen_window);
+/* Camera "orthographic" (OrthographicCamera::create, src/cameras/orthographic.rs:99-149): raster_to_camera from
+ * Transform::orthographic(0, 1), the screen window (NULL: from the frame aspect ratio) and the film's full resolution.  The
+ * reference's defaults are lensradius 0 and focaldistance 1e6. */
+int pbrt_host_camera_orthographic(PbrtHost* h, float lens_radius, float focal_distance, float shutter_open, float shutter_close,
+                                  const float* screen_window);
+/* Camera "environment" (EnvironmentCamera::create, src/cameras/environment.rs:44-90): camera_to_world, the shutter and the film's
+ * full resolution; it reads no screen window and no lens.  Call after pbrt_host_film. */
+int pbrt_host_camera_environment(PbrtHost* h, float shutter_open, float shutter_close);
 int pbrt_host_sampler_sobol(PbrtHost* h, int pixel_samples);
 /* Sampler "halton" (src/samplers/halton.rs:162-172), the reference's default sampler; any pixel_samples >= 1. */
 int pbrt_host_sampler_halton(PbrtHost* h, int pixel_samples, int sample_at_pixel_center);
@@ -121,6 +130,8 @@ const PbrtSceneDesc* pbrt_host_scene_desc(const PbrtHost* h);
 const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h);
 /* The motion description of the built scene, NULL when nothing in it is animated. */
 const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h);
+/* The camera model of the built scene (its kind and Film.full_resolution) for pbrt_gpu_scene_create_camera. */
+const PbrtCameraModel* pbrt_host_camera_model(const PbrtHost* h);
 
 /* Integrator::render(scene, num_threads): uploads the scene, renders pixel_rect (NULL = whole sample bounds) on `device`
  * through pbrt_gpu_render, and merges the result into the Film like merge_film_tile. */

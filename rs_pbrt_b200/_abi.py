@@ -84,6 +84,13 @@ class PbrtMotionDesc(C.Structure):
     _fields_ = [("camera", C.POINTER(PbrtAnimatedTransform)), ("instances", C.POINTER(PbrtAnimatedTransform))]
 
 
+PBRT_CAMERA_PERSPECTIVE, PBRT_CAMERA_ORTHOGRAPHIC, PBRT_CAMERA_ENVIRONMENT = 0, 1, 2
+
+
+class PbrtCameraModel(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("full_resolution", C.c_uint32 * 2)]
+
+
 class PbrtRenderParams(C.Structure):
     _fields_ = [("sample_bounds", C.c_int32 * 4), ("cropped_pixel_bounds", C.c_int32 * 4), ("pixel_bounds", C.c_int32 * 4),
                 ("filter_radius", C.c_float * 2), ("filter_table", C.c_float * 256), ("max_sample_luminance", C.c_float),
@@ -105,9 +112,9 @@ class PbrtStats(C.Structure):
 GPU_SYMBOLS = ["pbrt_gpu_scene_create", "pbrt_gpu_scene_destroy", "pbrt_gpu_scene_bytes", "pbrt_gpu_render", "pbrt_gpu_render_device", "pbrt_gpu_render_samples",
                "pbrt_gpu_render_tiles_device", "pbrt_gpu_render_multi", "pbrt_gpu_host_register", "pbrt_gpu_host_unregister",
                "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2",
-               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate", "pbrt_gpu_scene_create_multi"]
+               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate", "pbrt_gpu_scene_create_multi", "pbrt_gpu_scene_create_camera"]
 HOST_SYMBOLS = ["pbrt_host_new", "pbrt_host_free", "pbrt_host_last_error", "pbrt_host_add_material", "pbrt_host_add_material_mix", "pbrt_host_add_trianglemesh",
-                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
+                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_camera_orthographic", "pbrt_host_camera_environment", "pbrt_host_camera_model", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
                 "pbrt_host_integrator_path", "pbrt_host_world_end", "pbrt_host_scene_desc", "pbrt_host_render_params", "pbrt_host_render",
                 "pbrt_host_film_rgbw", "pbrt_host_film_clear", "pbrt_host_film_add_rgbw", "pbrt_host_film_rgb", "pbrt_host_write_image",
                 "pbrt_host_bvh_build"]
@@ -137,6 +144,8 @@ def bind(L):
     L.pbrt_gpu_scene_create.argtypes = [C.POINTER(PbrtSceneDesc), C.c_int, C.POINTER(vp)]
     L.pbrt_gpu_scene_create_motion.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.c_int, C.POINTER(vp)]
     L.pbrt_gpu_scene_create_multi.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(C.c_int), C.c_uint32, C.POINTER(vp)]
+    L.pbrt_gpu_scene_create_camera.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(PbrtCameraModel), C.POINTER(C.c_int), C.c_uint32,
+                                               C.POINTER(vp)]
     L.pbrt_gpu_kat_animated_interpolate.argtypes = [C.c_int, C.POINTER(PbrtAnimatedTransform), C.c_uint32, fp, fp, fp]
     L.pbrt_gpu_scene_destroy.argtypes = [vp]
     L.pbrt_gpu_scene_destroy.restype = None
@@ -176,6 +185,10 @@ def bind(L):
     L.pbrt_host_motion_desc.restype = C.POINTER(PbrtMotionDesc)
     L.pbrt_host_film.argtypes = [vp, C.c_int, C.c_int, fp, C.c_char_p, C.c_float, C.c_float, C.c_float, C.c_float]
     L.pbrt_host_camera_perspective.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, fp]
+    L.pbrt_host_camera_orthographic.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, fp]
+    L.pbrt_host_camera_environment.argtypes = [vp, C.c_float, C.c_float]
+    L.pbrt_host_camera_model.argtypes = [vp]
+    L.pbrt_host_camera_model.restype = C.POINTER(PbrtCameraModel)
     L.pbrt_host_sampler_sobol.argtypes = [vp, C.c_int]
     L.pbrt_host_sampler_halton.argtypes = [vp, C.c_int, C.c_int]
     L.pbrt_host_integrator_ao.argtypes = [vp, C.c_int, C.c_int]

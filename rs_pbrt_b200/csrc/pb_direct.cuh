@@ -184,6 +184,23 @@ PB_D bool direct_specular(const DScene& sc, const DPaths& ps, const DDirect& dd,
     return false;
 }
 
+// The first iteration's start of every camera sample, for camera rays WITHOUT a differential (the environment camera,
+// environment.rs:106: its first hits look textures up at level 0, like any later ray's): what k_direct_step does when `first` is set,
+// but with cur_has_diff = 0.  k_direct_step then runs its first iteration with first = 0 and reads this state.  (A second
+// instantiation of k_direct_step would have done the same, but it changes the compiler's inlining of the texture code shared with
+// k_texture and the alpha-tested k_trace, and with it their code.)
+__global__ void __launch_bounds__(128) k_direct_start_nodiff(DScene sc, DPaths ps, DDirect dd, BatchInfo bi) {
+    const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
+    if (slot >= bi.n_pixels * bi.n_samples) return;
+    const uint32_t state = (__float_as_uint(ps.L[slot].w) & PF_HAS_RAY) ? DS_WAIT_TRACE : DS_DONE;
+    dd.state[slot] = state;
+    dd.depth[slot] = 0;
+    dd.arr_off[slot] = 0u;
+    dd.nee_depth[slot] = -1;
+    if (sc.n_textures) dd.cur_has_diff[slot] = 0u;
+    if (state == DS_DONE) ps.L[slot] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
 __global__ void __launch_bounds__(128) k_direct_step(DScene sc, DRender rp, DPaths ps, DDirect dd, BatchInfo bi, const uint32_t* __restrict__ nib, uint32_t first,
                                                      float4* __restrict__ rays, uint32_t* __restrict__ d_nrays, uint32_t* __restrict__ d_active,
                                                      uint32_t* __restrict__ d_error, const uint32_t* __restrict__ prev_active) {

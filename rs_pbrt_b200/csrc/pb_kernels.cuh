@@ -100,13 +100,16 @@ struct BatchInfo {
 };
 
 // -----------------------------------------------------------------------------------------------
-// k_raygen: integrator.rs:123-144, sampler.rs:85-95, sobol.rs:110-138, perspective.rs:190-280
+// k_raygen: integrator.rs:123-144, sampler.rs:85-95, sobol.rs:110-138, and the camera's generate_ray_differential
+// (perspective.rs:190-280, orthographic.rs:156-230, environment.rs:92-116).
 // CAM_MOTION: the camera is animated (cam_mo); a static camera's instantiation never reads cam_mo.
-template <bool CAM_MOTION>
+// CAM_KIND: PbrtCameraKind.  env_res: Film.full_resolution as floats, read by the environment camera only.
+template <bool CAM_MOTION, int CAM_KIND>
 __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps, BatchInfo bi, const uint32_t* __restrict__ nib, uint32_t n_chunks,
                                                const uint64_t* __restrict__ vdc, const uint64_t* __restrict__ vdci, uint32_t* __restrict__ queue,
                                                uint32_t* __restrict__ d_count, float4* __restrict__ rays, uint32_t* __restrict__ d_nrays,
-                                               DCounters* cnt, const DMotion cam_mo) {
+                                               DCounters* cnt, const DMotion cam_mo, const float2 env_res) {
+    constexpr bool ORTHO = CAM_KIND == PBRT_CAMERA_ORTHOGRAPHIC, ENV = CAM_KIND == PBRT_CAMERA_ENVIRONMENT;
     __shared__ uint64_t s_vdc[52], s_vdci[52];
     if (threadIdx.x < 52) {
         uint32_t m = rp.log2_res;
@@ -165,13 +168,21 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
             V3 pc = mk3(xp, yp, zp);
             if (wp != 1.0f) { float inv = 1.0f / wp; pc = mk3(inv * xp, inv * yp, inv * zp); }
             V3 o = mk3(0.0f, 0.0f, 0.0f), d = norm3(pc);
+            if (ORTHO) { o = pc; d = mk3(0.0f, 0.0f, 1.0f); }  // orthographic.rs:165-176
+            if (ENV) {  // environment.rs:93-100 (f32 sin / cos: the glibc restatement)
+                const float theta = PB_PI * p_film.y / env_res.y, phi = 2.0f * PB_PI * p_film.x / env_res.x;
+                float st, ct, sp, cp;
+                sincos_rn(theta, st, ct);
+                sincos_rn(phi, sp, cp);
+                d = mk3(st * cp, ct, st * sp);
+            }
             (void)time;  // ray.time only selects an animated transform; static cameras ignore it
             float c2w_t[16];
             if (CAM_MOTION) {  // AnimatedTransform::transform_ray (transform.rs:2114-2124) at ray.time = lerp(sample.time, shutter) (perspective.rs:226)
                 float c2w_inv_t[16];
                 motion_interpolate(cam_mo, lerpf(time, sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
             }
-            if (sc.lens_radius > 0.0f) {
+            if (!ENV && sc.lens_radius > 0.0f) {  // (the same thin lens for the orthographic camera, orthographic.rs:177-188)
                 float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
                 pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
                 float ft = sc.focal_distance / d.z;
@@ -193,11 +204,24 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
                 float dt = dot3(abs3(dw), o_err) / ls;
                 ow = ow + dw * dt;
             }
-            if (ps.ray_diff) {  // textured scenes: the ray differential (perspective.rs:205-271), through camera_to_world (transform.rs:550-556), scaled (integrator.rs:140-144)
+            // textured scenes: the ray differential (perspective.rs:205-271), through camera_to_world (transform.rs:550-556), scaled
+            // (integrator.rs:140-144).  The environment camera makes none (environment.rs:106).
+            if (!ENV && ps.ray_diff) {
                 const V3 dxc = mk3(sc.dx_camera[0], sc.dx_camera[1], sc.dx_camera[2]), dyc = mk3(sc.dy_camera[0], sc.dy_camera[1], sc.dy_camera[2]);
                 V3 rxo = mk3(0.0f, 0.0f, 0.0f), ryo = rxo;
                 V3 rxd = norm3(pc + dxc), ryd = norm3(pc + dyc);
-                if (sc.lens_radius > 0.0f) {
+                if (ORTHO) {  // orthographic.rs:189-226
+                    rxo = o + dxc; ryo = o + dyc; rxd = d; ryd = d;
+                    if (sc.lens_radius > 0.0f) {
+                        // ft of the refracted ray.d, and one focus point (from dx_camera) for both differentials: ry == rx, as written
+                        float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
+                        pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
+                        const float ft = sc.focal_distance / d.z;
+                        const V3 p_focus = pc + dxc + mk3(0.0f, 0.0f, 1.0f) * ft;
+                        rxo = mk3(pl2.x, pl2.y, 0.0f); ryo = rxo;
+                        rxd = norm3(p_focus - rxo); ryd = norm3(p_focus - ryo);
+                    }
+                } else if (sc.lens_radius > 0.0f) {
                     float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
                     pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
                     const V3 dx = norm3(pc + dxc);

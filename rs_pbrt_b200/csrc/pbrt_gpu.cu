@@ -565,8 +565,10 @@ struct PbrtScene {
     DevBuf<float> ewa_lut;
     std::vector<Sp> h_env_power;  // per light: lmap.lookup((.5,.5), .5) for InfiniteAreaLight::power
     bool has_null_material = false;
-    bool cam_motion = false;  // the camera is animated: k_raygen<true> interpolates cam_mo at each sample's time
+    bool cam_motion = false;  // the camera is animated: k_raygen<true, ..> interpolates cam_mo at each sample's time
     DMotion cam_mo;
+    uint32_t cam_kind = PBRT_CAMERA_PERSPECTIVE;  // PbrtCameraKind: k_raygen's second template argument
+    float2 env_res = {0.0f, 0.0f};                // the environment camera's Film.full_resolution
     int light_level = 0;  // light level of the kernels that sample lights (pb_interaction.cuh): 0 = area lights only, 1 = any but image lights, 2 = with them
     uint32_t class_mask = 0;  // bit c: some material has shading class c (1..8: a single lobe of kind c - 1; 9: Lambert + microfacet reflection; 10..15: everything else)
     size_t upload_bytes = 0;
@@ -741,6 +743,13 @@ static bool enable_peer_access(int from, int to) {
     return e == cudaErrorPeerAccessAlreadyEnabled;
 }
 
+// k_raygen's instantiation for a scene's camera: its kind, animated or not
+static decltype(&k_raygen<false, PBRT_CAMERA_PERSPECTIVE>) raygen_kernel(const PbrtScene* sc) {
+    if (sc->cam_kind == PBRT_CAMERA_ORTHOGRAPHIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ORTHOGRAPHIC> : k_raygen<false, PBRT_CAMERA_ORTHOGRAPHIC>;
+    if (sc->cam_kind == PBRT_CAMERA_ENVIRONMENT) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ENVIRONMENT> : k_raygen<false, PBRT_CAMERA_ENVIRONMENT>;
+    return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_PERSPECTIVE> : k_raygen<false, PBRT_CAMERA_PERSPECTIVE>;
+}
+
 // ---- scene creation --------------------------------------------------------------------------------------------------------------
 // pbrt_gpu_scene_create, _create_motion and _create_multi are one code path in two phases.  scene_prepare validates the description
 // and makes every host-side table once: lobe lists and shading classes, texture / environment / light-map pyramids and their
@@ -787,6 +796,8 @@ struct ScenePrep {
     int light_level = 0;
     uint32_t class_mask = 0;
     DMotion cam_mo;
+    uint32_t cam_kind = PBRT_CAMERA_PERSPECTIVE;
+    float2 env_res = {0.0f, 0.0f};
 };
 
 // The host-side passes run on all cores (a 4.3 M-triangle scene is re-uploaded on every end-to-end step).
@@ -825,9 +836,17 @@ static int tri_fail(int code) {
     return fail(PBRT_E_INVALID, "instance index out of range");
 }
 
-static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, ScenePrep& P) {
+static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, ScenePrep& P) {
     P.desc = desc;
     std::memset(&P.cam_mo, 0, sizeof P.cam_mo);
+    if (camera) {
+        if (camera->kind != PBRT_CAMERA_PERSPECTIVE && camera->kind != PBRT_CAMERA_ORTHOGRAPHIC && camera->kind != PBRT_CAMERA_ENVIRONMENT)
+            return fail(PBRT_E_UNSUPPORTED, "camera kind outside the GPU path (perspective, orthographic and environment are on it)");
+        if (camera->kind == PBRT_CAMERA_ENVIRONMENT && (camera->full_resolution[0] == 0 || camera->full_resolution[1] == 0))
+            return fail(PBRT_E_INVALID, "environment camera with a zero full_resolution");
+        P.cam_kind = camera->kind;
+        P.env_res = make_float2((float)camera->full_resolution[0], (float)camera->full_resolution[1]);
+    }
     if (motion && motion->instances) {
         if (desc->n_instances && !desc->instances) return fail(PBRT_E_INVALID, "null instance array in scene description");
         for (uint32_t i = 0; i < desc->n_instances; ++i) {
@@ -1291,7 +1310,13 @@ static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion
     d.n_inf = n_inf;
     d.n_instances = desc->n_instances;
     d.n_textures = desc->n_textures;
-    {  // dx_camera / dy_camera, PerspectiveCamera::new (perspective.rs:82-99)
+    if (P.cam_kind == PBRT_CAMERA_ORTHOGRAPHIC) {  // dx_camera / dy_camera, OrthographicCamera::new (orthographic.rs:75-84): transform_vector
+        const float* m = desc->camera.raster_to_camera;
+        d.dx_camera[0] = m[0] * 1.0f + m[1] * 0.0f + m[2] * 0.0f; d.dx_camera[1] = m[4] * 1.0f + m[5] * 0.0f + m[6] * 0.0f;
+        d.dx_camera[2] = m[8] * 1.0f + m[9] * 0.0f + m[10] * 0.0f;
+        d.dy_camera[0] = m[0] * 0.0f + m[1] * 1.0f + m[2] * 0.0f; d.dy_camera[1] = m[4] * 0.0f + m[5] * 1.0f + m[6] * 0.0f;
+        d.dy_camera[2] = m[8] * 0.0f + m[9] * 1.0f + m[10] * 0.0f;
+    } else {  // dx_camera / dy_camera, PerspectiveCamera::new (perspective.rs:82-99)
         auto r2c = [&](float x, float y) {
             const float* m = desc->camera.raster_to_camera;
             V3 r = mk3(m[0] * x + m[1] * y + m[2] * 0.0f + m[3], m[4] * x + m[5] * y + m[6] * 0.0f + m[7], m[8] * x + m[9] * y + m[10] * 0.0f + m[11]);
@@ -1531,12 +1556,15 @@ static int build_finish(const ScenePrep& P, std::vector<SceneBuild>& builds, uin
     // a camera whose keyframes are equal takes the static kernels: interpolate() would hand back the start transform at every time
     sc->cam_motion = P.cam_mo.actually_animated != 0;
     sc->cam_mo = P.cam_mo;
+    sc->cam_kind = P.cam_kind;
+    sc->env_res = P.env_res;
     CK(cudaDeviceSynchronize());
     return PBRT_OK;
 }
 
 // The scene on devices[0..n) (distinct, already checked by the caller): out[k] is the replica on devices[k], or every out[k] is null.
-static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n, PbrtScene** out) {
+static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices, uint32_t n,
+                         PbrtScene** out) {
     static const int timing = getenv("PB_TIMING") ? atoi(getenv("PB_TIMING")) : 0;  // 1: every call; 2: only calls slower than 100 ms
     const auto t_enter = std::chrono::steady_clock::now();
     std::string timing_log;
@@ -1550,7 +1578,7 @@ static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion
         if (mode == 2 && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() > 100.0) fputs(log.c_str(), stderr); } } slow_dump{timing_log, t_enter, timing};
     for (uint32_t k = 0; k < n; ++k) out[k] = nullptr;
     ScenePrep P;
-    int rc = scene_prepare(desc, motion, P);
+    int rc = scene_prepare(desc, motion, camera, P);
     if (rc != PBRT_OK) return rc;
     since("host preparation");
     for (uint32_t k = 0; k < n; ++k) {
@@ -1625,22 +1653,27 @@ extern "C" {
 
 int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out) {
     if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    return create_scenes(desc, nullptr, &device, 1, out);
+    return create_scenes(desc, nullptr, nullptr, &device, 1, out);
 }
 
 int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out) {
     if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    return create_scenes(desc, motion, &device, 1, out);
+    return create_scenes(desc, motion, nullptr, &device, 1, out);
 }
 
 int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n_devices, PbrtScene** out) {
+    return pbrt_gpu_scene_create_camera(desc, motion, nullptr, devices, n_devices, out);
+}
+
+int pbrt_gpu_scene_create_camera(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices,
+                                 uint32_t n_devices, PbrtScene** out) {
     if (!desc || !devices || !out || n_devices == 0) return fail(PBRT_E_INVALID, "null argument or no device");
     for (uint32_t k = 0; k < n_devices; ++k) out[k] = nullptr;
     if (n_devices > 16) return fail(PBRT_E_UNSUPPORTED, "more than 16 devices");
     for (uint32_t k = 0; k < n_devices; ++k)
         for (uint32_t j = 0; j < k; ++j)
             if (devices[j] == devices[k]) return fail(PBRT_E_INVALID, "a device is listed twice (one replica per device)");
-    return create_scenes(desc, motion, devices, n_devices, out);
+    return create_scenes(desc, motion, camera, devices, n_devices, out);
 }
 
 int pbrt_gpu_host_register(const void* ptr, uint64_t bytes) {
@@ -1935,9 +1968,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+                const auto raygen = raygen_kernel(sc);
                 raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, sc->nib.p, std::max(raygen_chunks, dd.n_chunks), sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count,
-                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo);
+                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo, sc->env_res);
                 launches++;
                 // the recursion's length is decided on the device (the active word = camera samples that still need an iteration).  The
                 // host reads that word poll_lag() iterations late (see there: 0 by default, measured): with a lag of 1 iteration i + 1 is
@@ -1953,7 +1986,12 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                     cudaEvent_t e, g;
                     CK(scr->event(&e)); CK(scr->event(&g));
                     CK(cudaEventRecord(e, st));
-                    k_direct_step<<<(n + 127) / 128, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, iter == 0 ? 1u : 0u, X.rays.p, d_nrays, d_active, d_err, d_prev);
+                    const bool env_start = iter == 0 && sc->cam_kind == PBRT_CAMERA_ENVIRONMENT;  // camera rays without a differential
+                    if (env_start) {
+                        k_direct_start_nodiff<<<(n + 127) / 128, 128, 0, st>>>(dsc, ps, dd, bi);
+                        launches++;
+                    }
+                    k_direct_step<<<(n + 127) / 128, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, iter == 0 && !env_start ? 1u : 0u, X.rays.p, d_nrays, d_active, d_err, d_prev);
                     const uint64_t total = (uint64_t)n * n_nee;
                     const unsigned nee_grid = (unsigned)((total + 127) / 128);
                     if (sc->light_level >= 2) k_direct_nee<2><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
@@ -2042,9 +2080,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+                const auto raygen = raygen_kernel(sc);
                 raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count, X.rays.p, d_nrays,
-                                                        sc->counters.p, sc->cam_mo);
+                                                        sc->counters.p, sc->cam_mo, sc->env_res);
                 launches++;
                 int rc = trace();
                 if (rc != PBRT_OK) return rc;
@@ -2370,8 +2408,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             k_sort<<<sm_count * 8, 256, 0, s>>>(sc->d, V.ps, V.grid, spatial ? 1u : 0u, rp.instancing, X.queue[cur].p, c_in, X.cls_queue.p, (uint32_t)cap, cls_now, c_out,
                                                 V.d_nrays);
             launches++;
-            if (textured) {  // V.iter == 1: the rays just traced are the camera rays, the only ones with differentials
-                k_texture<<<sm_count * 8, 128, 0, s>>>(sc->d, rp, V.ps, X.queue[cur].p, c_in, V.iter == 1 ? 1u : 0u);
+            if (textured) {  // V.iter == 1: the rays just traced are the camera rays, the only ones with differentials (none from an environment camera)
+                k_texture<<<sm_count * 8, 128, 0, s>>>(sc->d, rp, V.ps, X.queue[cur].p, c_in, V.iter == 1 && sc->cam_kind != PBRT_CAMERA_ENVIRONMENT ? 1u : 0u);
                 launches++;
             }
             if (spatial) {
@@ -2443,9 +2481,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             // ray count, ray cursor, both sets of class counts (and the voxel requests): from here on the kernels reset them for each other
             CK(cudaMemsetAsync(V.d_nrays, 0, (5 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
             if (spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
-            const auto raygen = sc->cam_motion ? k_raygen<true> : k_raygen<false>;
+            const auto raygen = raygen_kernel(sc);
             raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays,
-                                                      sc->counters.p, sc->cam_mo);
+                                                      sc->counters.p, sc->cam_mo, sc->env_res);
             launches++;
             return PBRT_OK;
         };

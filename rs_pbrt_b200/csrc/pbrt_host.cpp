@@ -315,6 +315,7 @@ struct PbrtHost {
     float max_sample_luminance = std::numeric_limits<float>::infinity();
     bool have_camera = false;
     PbrtCamera cam;
+    PbrtCameraModel cam_model = {PBRT_CAMERA_PERSPECTIVE, {0, 0}};
     int pixel_samples = 16;
     uint32_t sampler = PBRT_SAMPLER_SOBOL;
     bool sample_at_pixel_center = false;
@@ -744,6 +745,45 @@ int pbrt_host_camera_perspective(PbrtHost* h, float fov, float lens_radius, floa
     std::memcpy(h->cam.camera_to_world, h->camera_to_world.m, 64);
     h->cam.lens_radius = lens_radius; h->cam.focal_distance = focal_distance;
     h->cam.shutter_open = shutter_open; h->cam.shutter_close = shutter_close;
+    h->cam_model = PbrtCameraModel{PBRT_CAMERA_PERSPECTIVE, {(uint32_t)h->xres, (uint32_t)h->yres}};
+    h->have_camera = true;
+    return 0;
+}
+
+int pbrt_host_camera_orthographic(PbrtHost* h, float lens_radius, float focal_distance, float shutter_open, float shutter_close,
+                                  const float* screen_window) {  // OrthographicCamera::create / new, orthographic.rs:47-149
+    if (!h) return hfail(PBRT_E_INVALID, "null argument");
+    float frame = (float)h->xres / (float)h->yres;
+    float sw[4];  // xmin, xmax, ymin, ymax
+    if (frame > 1.0f) { sw[0] = -frame; sw[1] = frame; sw[2] = -1.0f; sw[3] = 1.0f; }
+    else { sw[0] = -1.0f; sw[1] = 1.0f; sw[2] = -1.0f / frame; sw[3] = 1.0f / frame; }
+    if (screen_window) std::memcpy(sw, screen_window, 16);
+    const float z_near = 0.0f, z_far = 1.0f;  // Transform::orthographic(0, 1), transform.rs:452-460
+    Xf camera_to_screen = xf_mul(xf_scale(1.0f, 1.0f, 1.0f / (z_far - z_near)), xf_translate(0.0f, 0.0f, -z_near));
+    Xf scale1 = xf_scale((float)h->xres, (float)h->yres, 1.0f);
+    Xf scale2 = xf_scale(1.0f / (sw[1] - sw[0]), 1.0f / (sw[2] - sw[3]), 1.0f);
+    Xf translate = xf_translate(-sw[0], -sw[3], 0.0f);
+    Xf screen_to_raster = xf_mul(xf_mul(scale1, scale2), translate);
+    Xf raster_to_screen{screen_to_raster.inv, screen_to_raster.m};
+    Xf c2s_inv{camera_to_screen.inv, camera_to_screen.m};
+    Xf raster_to_camera = xf_mul(c2s_inv, raster_to_screen);
+    std::memcpy(h->cam.raster_to_camera, raster_to_camera.m.m, 64);
+    std::memcpy(h->cam.camera_to_world, h->camera_to_world.m, 64);
+    h->cam.lens_radius = lens_radius; h->cam.focal_distance = focal_distance;
+    h->cam.shutter_open = shutter_open; h->cam.shutter_close = shutter_close;
+    h->cam_model = PbrtCameraModel{PBRT_CAMERA_ORTHOGRAPHIC, {(uint32_t)h->xres, (uint32_t)h->yres}};
+    h->have_camera = true;
+    return 0;
+}
+
+int pbrt_host_camera_environment(PbrtHost* h, float shutter_open, float shutter_close) {  // EnvironmentCamera::create, environment.rs:44-90
+    if (!h) return hfail(PBRT_E_INVALID, "null argument");
+    const M4 ident = m4_identity();  // the environment camera has no raster_to_camera and no lens
+    std::memcpy(h->cam.raster_to_camera, ident.m, 64);
+    std::memcpy(h->cam.camera_to_world, h->camera_to_world.m, 64);
+    h->cam.lens_radius = 0.0f; h->cam.focal_distance = 1e30f;
+    h->cam.shutter_open = shutter_open; h->cam.shutter_close = shutter_close;
+    h->cam_model = PbrtCameraModel{PBRT_CAMERA_ENVIRONMENT, {(uint32_t)h->xres, (uint32_t)h->yres}};
     h->have_camera = true;
     return 0;
 }
@@ -1001,11 +1041,12 @@ int pbrt_host_world_end(PbrtHost* h, uint32_t max_prims_in_node, int n_threads) 
 const PbrtSceneDesc* pbrt_host_scene_desc(const PbrtHost* h) { return (h && h->built) ? &h->desc : nullptr; }
 const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h) { return (h && h->built && h->motion.camera) ? &h->motion : nullptr; }
 const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h) { return (h && h->built) ? &h->rp : nullptr; }
+const PbrtCameraModel* pbrt_host_camera_model(const PbrtHost* h) { return (h && h->built) ? &h->cam_model : nullptr; }
 
 int pbrt_host_render(PbrtHost* h, int device, const int32_t* pixel_rect, PbrtStats* stats) {
     if (!h || !h->built) return hfail(PBRT_E_INVALID, "pbrt_host_world_end has not run");
     PbrtScene* sc = nullptr;
-    int rc = pbrt_gpu_scene_create_motion(&h->desc, pbrt_host_motion_desc(h), device, &sc);
+    int rc = pbrt_gpu_scene_create_camera(&h->desc, pbrt_host_motion_desc(h), pbrt_host_camera_model(h), &device, 1, &sc);
     if (rc != PBRT_OK) return hfail(rc, pbrt_gpu_last_error());
     const int32_t* rect = pixel_rect ? pixel_rect : h->rp.sample_bounds;
     rc = pbrt_gpu_render(sc, &h->rp, rect, h->film.data(), stats);

@@ -229,6 +229,18 @@ class HostScene:
                                         screenwindow=None if sw is None else sw.copy())))
         self._ck(self.L.pbrt_host_camera_perspective(self.h, fov, lensradius, focaldistance, shutteropen, shutterclose, _fptr(sw)))
 
+    def camera_orthographic(self, lensradius=0.0, focaldistance=1e6, shutteropen=0.0, shutterclose=1.0, screenwindow=None):
+        """Camera "orthographic" (the reference's defaults); call after film()."""
+        sw = _f32(screenwindow)
+        self.log.append(("camera_orthographic", dict(lensradius=float(lensradius), focaldistance=float(focaldistance), shutteropen=float(shutteropen),
+                                                     shutterclose=float(shutterclose), screenwindow=None if sw is None else sw.copy())))
+        self._ck(self.L.pbrt_host_camera_orthographic(self.h, lensradius, focaldistance, shutteropen, shutterclose, _fptr(sw)))
+
+    def camera_environment(self, shutteropen=0.0, shutterclose=1.0):
+        """Camera "environment": a lat-long view of the whole sphere around camera_to_world's origin; call after film()."""
+        self.log.append(("camera_environment", dict(shutteropen=float(shutteropen), shutterclose=float(shutterclose))))
+        self._ck(self.L.pbrt_host_camera_environment(self.h, shutteropen, shutterclose))
+
     def sampler(self, pixelsamples=16, name="sobol", samplepixelcenter=False):
         """Sampler "sobol" (pixelsamples rounded up to a power of two) or "halton"."""
         self.log.append(("sampler", dict(pixelsamples=int(pixelsamples), name=name, samplepixelcenter=bool(samplepixelcenter))))
@@ -307,6 +319,12 @@ class HostScene:
         p = self.L.pbrt_host_motion_desc(self.h)
         return p if p else None
 
+    @property
+    def camera_model(self):
+        """The PbrtCameraModel of the built scene (kind and full film resolution), for GpuScene(camera=...) and create_multi."""
+        p = self.L.pbrt_host_camera_model(self.h)
+        return p if p else None
+
     def film_shape(self):
         cb = self.params.contents.cropped_pixel_bounds
         return (cb[3] - cb[1], cb[2] - cb[0])
@@ -342,12 +360,16 @@ class HostScene:
 
 class GpuScene:
     """A scene resident on one GPU: pbrt_gpu_scene_create / render / intersect (include/pbrt_gpu.h).  `motion`: a PbrtMotionDesc (or a
-    pointer to one, e.g. HostScene.motion) for pbrt_gpu_scene_create_motion."""
+    pointer to one, e.g. HostScene.motion) for pbrt_gpu_scene_create_motion.  `camera`: a PbrtCameraModel (or a pointer to one, e.g.
+    HostScene.camera_model) for pbrt_gpu_scene_create_camera; None is the perspective camera."""
 
-    def __init__(self, desc, device=0, lib=None, motion=None):
+    def __init__(self, desc, device=0, lib=None, motion=None, camera=None):
         self.L = lib if lib is not None else _abi.load()  # `lib`: tests may pass another build of the same C ABI
         self.handle = C.c_void_p()
-        if motion is not None:
+        if camera is not None:
+            dev = C.c_int(device)
+            rc = self.L.pbrt_gpu_scene_create_camera(desc, _ptr(motion), _ptr(camera), C.byref(dev), 1, C.byref(self.handle))
+        elif motion is not None:
             rc = self.L.pbrt_gpu_scene_create_motion(desc, motion if isinstance(motion, C._Pointer) else C.byref(motion), device, C.byref(self.handle))
         else:
             rc = self.L.pbrt_gpu_scene_create(desc, device, C.byref(self.handle))
@@ -456,15 +478,22 @@ def unpin_description(handle):
         L.pbrt_gpu_host_unregister(C.c_void_p(a))
 
 
-def create_multi(desc, devices, motion=None, lib=None):
+def _ptr(x):
+    return x if x is None or isinstance(x, C._Pointer) else C.pointer(x)
+
+
+def create_multi(desc, devices, motion=None, lib=None, camera=None):
     """pbrt_gpu_scene_create_multi: the scene on every device of `devices` in one call, each large array crossing PCIe once; returns one
-    GpuScene per device, in the order given.  `motion`: as for GpuScene."""
+    GpuScene per device, in the order given.  `motion`, `camera`: as for GpuScene (a camera model goes through
+    pbrt_gpu_scene_create_camera)."""
     L = lib if lib is not None else _abi.load()
     devs = (C.c_int * len(devices))(*[int(d) for d in devices])
     handles = (C.c_void_p * max(len(devices), 1))()
-    if motion is not None and not isinstance(motion, C._Pointer):
-        motion = C.pointer(motion)
-    rc = L.pbrt_gpu_scene_create_multi(desc, motion, devs, len(devices), handles)
+    motion = _ptr(motion)
+    if camera is not None:
+        rc = L.pbrt_gpu_scene_create_camera(desc, motion, _ptr(camera), devs, len(devices), handles)
+    else:
+        rc = L.pbrt_gpu_scene_create_multi(desc, motion, devs, len(devices), handles)
     if rc != 0:
         raise PbrtError(rc, L.pbrt_gpu_last_error().decode())
     out = []

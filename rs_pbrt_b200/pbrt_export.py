@@ -275,8 +275,8 @@ def write(h, path, ply_threshold=2000):
             camera_end = a["m"]
         elif name == "film":
             film = a
-        elif name == "camera":
-            camera = a
+        elif name in ("camera", "camera_orthographic", "camera_environment"):
+            camera = dict(a, kind=name)
         elif name == "sampler":
             sampler = a
         elif name == "integrator":
@@ -292,7 +292,13 @@ def write(h, path, ply_threshold=2000):
     elif look:
         pre.append(look)
     c = camera or {}
-    s = 'Camera "perspective" "float fov" [%r]' % c.get("fov", 90.0)
+    kind = c.get("kind", "camera")
+    if kind == "camera_orthographic":
+        s = 'Camera "orthographic"'
+    elif kind == "camera_environment":
+        s = 'Camera "environment"'
+    else:
+        s = 'Camera "perspective" "float fov" [%r]' % c.get("fov", 90.0)
     if (c.get("shutteropen", 0.0), c.get("shutterclose", 1.0)) != (0.0, 1.0):
         s += ' "float shutteropen" [%r] "float shutterclose" [%r]' % (c["shutteropen"], c["shutterclose"])
     if c.get("lensradius", 0.0) > 0.0:

@@ -81,7 +81,8 @@ def projector_transform(pos, target, up=(0.0, 1.0, 0.0)):
 
 def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filter="box", xwidth=0.5, ywidth=0.5, lensradius=0.0,
                 focaldistance=1e6, n_threads=8, crop=None, materials="matte", lights="area", sampler="sobol", samplepixelcenter=False, integrator="path", textures=None, lightsamples=1,
-                alpha=None, quantize_textures=False, camera_end=None, shutter=(0.0, 1.0), transform_times=(0.0, 1.0)):
+                alpha=None, quantize_textures=False, camera_end=None, shutter=(0.0, 1.0), transform_times=(0.0, 1.0), camera="perspective",
+                screenwindow=None):
     """Canonical Cornell box: 5 walls, short and tall block, ceiling light quad (2 triangles => 2 area lights, so
     the spatial light distribution is active).  32 triangles.  `materials="mixed"` swaps the blocks to glass /
     metal and the floor to plastic for BxDF coverage ("translucent", "mix": TranslucentMaterial / MixMaterial on blocks, floor and back wall).  `lights`: "area" (the ceiling quad only), "delta" (plus a point, a spot
@@ -94,7 +95,9 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
     the Shape's "alpha" / "shadowalpha" float textures (triangle.rs:313-330,593-654): a leaf-like cut-out through an image mask (visible
     and shadow-casting only where the mask is non-zero), a card with a shadow-alpha mask only (fully visible, casts a shadow with holes)
     and a card with `"float alpha" 0` (never hit by anything).  `quantize_textures`: every image texel is rounded to a multiple of 1/255, so
-    that the scene equals its own .pbrt export (rs_pbrt reads images as 8-bit RGB; rs_pbrt_b200/pbrt_export.py)."""
+    that the scene equals its own .pbrt export (rs_pbrt reads images as 8-bit RGB; rs_pbrt_b200/pbrt_export.py).  `camera`:
+    "perspective", "orthographic" (a view of the box's front, 560 units high, unless `screenwindow` says otherwise; lensradius /
+    focaldistance apply) or "environment" (a lat-long view of everything around a point inside the box, near its open front)."""
     h = HostScene()
     if quantize_textures:
         _ti = h.texture_image
@@ -225,14 +228,37 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
         h.light_goniometric([30000.0, 28000.0, 24000.0], scale=[1.5, 1.5, 1.5], texels=gonio_map(), light_to_world=gonio_transform([278.0, 470.0, 279.5]))
     if lights == "projection":
         h.light_projection([60000.0, 60000.0, 60000.0], projector_slide(), fov=30.0, light_to_world=projector_transform([278.0, 300.0, 20.0], [300.0, 250.0, 555.0]))
-    h.look_at([278, 273, -800], [278, 273, 0], [0, 1, 0])
+    eye = _cornell_eye(camera)
+    h.look_at(eye, [eye[0], eye[1], eye[2] + 800.0], [0, 1, 0])
     _camera_motion(h, camera_end, transform_times)
     h.film(xres, yres, crop=crop, filter=filter, xwidth=xwidth, ywidth=ywidth)
-    h.camera(fov=39.3077, lensradius=lensradius, focaldistance=focaldistance, shutteropen=shutter[0], shutterclose=shutter[1])
+    if camera == "orthographic":
+        h.camera_orthographic(lensradius=lensradius, focaldistance=focaldistance, shutteropen=shutter[0], shutterclose=shutter[1],
+                              screenwindow=screenwindow if screenwindow is not None else _screen_window(xres, yres, 280.0))
+    elif camera == "environment":
+        h.camera_environment(shutteropen=shutter[0], shutterclose=shutter[1])
+    elif camera == "perspective":
+        h.camera(fov=39.3077, lensradius=lensradius, focaldistance=focaldistance, shutteropen=shutter[0], shutterclose=shutter[1], screenwindow=screenwindow)
+    else:
+        raise ValueError("camera outside the GPU path: %s" % camera)
     h.sampler(spp, name=sampler, samplepixelcenter=samplepixelcenter)
     _set_integrator(h, integrator, maxdepth, strategy)
     h.world_end(n_threads=n_threads)
     return h
+
+
+def _cornell_eye(camera):
+    """The Cornell box's eye: 800 units in front of the box, or 120 units inside it for the environment camera."""
+    return [278.0, 273.0, 120.0 if camera == "environment" else -800.0]
+
+
+def _screen_window(xres, yres, half):
+    """An orthographic screen window `half` units high either side of the view axis, widened by the frame's aspect ratio
+    (OrthographicCamera::create's default shape, orthographic.rs:112-129, scaled)."""
+    frame = xres / yres
+    if frame > 1.0:
+        return [-half * frame, half * frame, -half, half]
+    return [-half, half, -half / frame, half / frame]
 
 
 def look_at_matrix(eye, look, up):
@@ -261,7 +287,8 @@ def motion_cornell(xres=64, yres=64, spp=16, dolly=150.0, pan=0.0, shutter=(0.0,
     `pan` degrees about the vertical axis (a rotation keyframe: slerp); `shutter` = (shutteropen, shutterclose).  Other keyword
     arguments go to cornell_box (materials, lights, textures, lensradius, sampler, integrator, ...)."""
     a = np.radians(pan)
-    eye = [278.0, 273.0, -800.0 + dolly]
+    eye = _cornell_eye(kw.get("camera", "perspective"))
+    eye[2] += dolly
     look = [eye[0] + 800.0 * np.sin(a), 273.0, eye[2] + 800.0 * np.cos(a)]
     return cornell_box(xres=xres, yres=yres, spp=spp, camera_end=look_at_matrix(eye, look, [0, 1, 0]), shutter=shutter,
                        transform_times=transform_times, **kw)
@@ -412,12 +439,13 @@ def _fbm(u, v, rng, octaves=6):
 
 
 def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, with_normals=True, n_threads=8, crop=None, integrator="path",
-           dolly=0.0, extra_light=None):
+           dolly=0.0, extra_light=None, camera="perspective"):
     """Ganesha stand-in (config C3): an fBm-displaced, vertically stretched UV sphere of 2*n_side^2 triangles
     (n_side=1468 -> 4.31 M) with per-vertex normals, on a ground quad, lit by 3 rectangular area lights
     (6 light triangles); matte statue + plastic ground.  `dolly` != 0: the camera moves that far towards the statue over the
     shutter interval (motion blur).  `extra_light`: None, "point" or "goniometric" -- one more light at the same place above the statue
-    (the goniometric one turned, with gonio_map()): what the image lookup of a goniometric light costs."""
+    (the goniometric one turned, with gonio_map()): what the image lookup of a goniometric light costs.  `camera`: "perspective",
+    "orthographic" (a view 3.2 units high either side of the axis) or "environment" (the whole sphere around the same eye)."""
     rng = np.random.default_rng(seed)
     h = HostScene()
     body = h.material(_abi.MAT_MATTE, [0.62, 0.47, 0.33, 0.0])
@@ -468,7 +496,14 @@ def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, wi
         eye = np.array([0.0, 3.2, -7.5]) + dolly * np.array([0.0, -1.2, 7.5]) / np.linalg.norm([0.0, -1.2, 7.5])
         _camera_motion(h, look_at_matrix(eye, [0.0, 2.0, 0.0], [0, 1, 0]), (0.0, 1.0))
     h.film(xres, yres, crop=crop)
-    h.camera(fov=38.0)
+    if camera == "orthographic":
+        h.camera_orthographic(screenwindow=_screen_window(xres, yres, 3.2))
+    elif camera == "environment":
+        h.camera_environment()
+    elif camera == "perspective":
+        h.camera(fov=38.0)
+    else:
+        raise ValueError("camera outside the GPU path: %s" % camera)
     h.sampler(spp)
     _set_integrator(h, integrator, maxdepth, "spatial")
     h.world_end(n_threads=n_threads)
