@@ -24,7 +24,8 @@
  * (pbrt_gpu_render_tiles*) and the one-process multi-device render (pbrt_gpu_render_multi); within 4, the animated camera
  * (pbrt_gpu_scene_create_motion and its new structs: nothing that existed changed); within 4, goniometric and projection lights
  * (PBRT_LIGHT_GONIOMETRIC / PROJECTION and PbrtLight.fov in the former pad word); within 4, pbrt_gpu_scene_create_multi; within 4,
- * orthographic and environment cameras (pbrt_gpu_scene_create_camera, PbrtCameraModel).  Structs only ever grow at their end
+ * orthographic and environment cameras (pbrt_gpu_scene_create_camera, PbrtCameraModel); within 4, the realistic camera
+ * (pbrt_gpu_scene_create_lens, PbrtRealisticLens, PBRT_CAMERA_REALISTIC).  Structs only ever grow at their end
  * within a version step, and a zero-initialised new field means "as before".
  */
 #ifndef PBRT_GPU_H
@@ -401,18 +402,64 @@ int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc*
  *                 phi) from the origin.  The ray has NO differential (differential: None), so the first hit's texture lookups are
  *                 level-0 lookups, like a later bounce's.  raster_to_camera and the lens are not read.
  * full_resolution is Film.full_resolution {x, y}: the environment camera divides by it; the crop window does not change it.
- * An unknown kind (RealisticCamera included) is PBRT_E_UNSUPPORTED; an ENVIRONMENT model with a zero full_resolution is
- * PBRT_E_INVALID. */
-typedef enum PbrtCameraKind { PBRT_CAMERA_PERSPECTIVE = 0, PBRT_CAMERA_ORTHOGRAPHIC = 1, PBRT_CAMERA_ENVIRONMENT = 2 } PbrtCameraKind;
+ *   REALISTIC     RealisticCamera (src/cameras/realistic.rs:198-735): only through pbrt_gpu_scene_create_lens below, which also takes
+ *                 the lens system.
+ * full_resolution is Film.full_resolution {x, y}: the environment and realistic cameras divide by it; the crop window does not
+ * change it.  An unknown kind, and REALISTIC handed to pbrt_gpu_scene_create_camera, are PBRT_E_UNSUPPORTED; an ENVIRONMENT or
+ * REALISTIC model with a zero full_resolution is PBRT_E_INVALID. */
+typedef enum PbrtCameraKind {
+    PBRT_CAMERA_PERSPECTIVE = 0,
+    PBRT_CAMERA_ORTHOGRAPHIC = 1,
+    PBRT_CAMERA_ENVIRONMENT = 2,
+    PBRT_CAMERA_REALISTIC = 3
+} PbrtCameraKind;
 typedef struct PbrtCameraModel {
     uint32_t kind;               /* PbrtCameraKind */
-    uint32_t full_resolution[2]; /* ENVIRONMENT: Film.full_resolution {x, y} */
+    uint32_t full_resolution[2]; /* ENVIRONMENT, REALISTIC: Film.full_resolution {x, y} */
 } PbrtCameraModel;
 /* pbrt_gpu_scene_create_multi with a camera model; camera == NULL is the perspective camera, motion may be NULL, and n_devices == 1
  * is a single scene.  pbrt_gpu_scene_create, _create_motion and _create_multi are this call with camera == NULL.  Errors as for
  * pbrt_gpu_scene_create_multi, and those of the camera model above. */
 int pbrt_gpu_scene_create_camera(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices,
                                  uint32_t n_devices, PbrtScene** out);
+
+/* ---- the realistic camera (ABI v4) ---------------------------------------------------------------------------------------------
+ * RealisticCamera (src/cameras/realistic.rs) as the caller has already built it: the library computes neither the focus nor the
+ * exit pupil, so it cannot disagree with the caller's CPU loop about them.  What a camera sample does (generate_ray_differential,
+ * :693-735, with generate_ray :198-251):
+ *   - the film point is (-x, y, 0) of Film::get_physical_extent().lerp(p_film / full_resolution) (film.rs:293-307, from diagonal);
+ *   - sample_exit_pupil (:656-688): bin min(63, floor(r / (diagonal / 2) * 64)), that bin's bounds lerped by p_lens and turned by
+ *     the film point's angle, on the plane z = the last element's thickness;
+ *   - trace_lenses_from_film (:266-327) from the film point to that point, through Transform::scale(1, 1, -1) both ways (origin
+ *     error offset included); then camera_to_world (animated or not, PbrtMotionDesc.camera) and a normalise;
+ *   - weight: simple_weighting ? cos^4(theta) * area / exit_pupil_bounds[0].area() : (shutter_close - shutter_open) * (cos^4(theta) *
+ *     area) / rear_z^2, cos(theta) the z of the normalised film ray, area that of the sample's bin; 0 when the ray vignettes;
+ *   - the differentials shift p_film by +0.05 (-0.05 when that vignettes) in x, then in y; when neither shift of one axis passes,
+ *     the whole sample's weight is 0.  So the shifted rays are always traced, textured scene or not.
+ * The integrator runs li only for a weight > 0 (integrator.rs:157): a vignetted sample adds L = 0 and counts its filter weight, so
+ * it darkens its pixel; PbrtStats.camera_rays counts the samples that were traced.  Every other field of the film (L * weight *
+ * filter weight, integrator.rs:186) follows.  pbrt_gpu_render_samples reports li's L, unweighted.  PbrtCamera.raster_to_camera,
+ * lens_radius and focal_distance are not read. */
+#define PBRT_MAX_LENS_ELEMENTS 32 /* element interfaces per lens; published prescriptions have about 6-16 */
+typedef struct PbrtLensElement {
+    float curvature_radius; /* metres, 0 = aperture stop */
+    float thickness;        /* metres; the last element's is the focused lens-film distance (focus_thick_lens, :483-499) */
+    float eta;              /* 0 = air */
+    float aperture_radius;  /* metres */
+} PbrtLensElement;
+typedef struct PbrtRealisticLens {
+    const PbrtLensElement* elements;  /* RealisticCamera.element_interfaces after construction, scene side first */
+    uint32_t n_elements;              /* 1 .. PBRT_MAX_LENS_ELEMENTS */
+    const float* exit_pupil_bounds;   /* RealisticCamera.exit_pupil_bounds: 64 x {pmin.x, pmin.y, pmax.x, pmax.y} */
+    float film_diagonal;              /* Film.diagonal, metres */
+    uint32_t simple_weighting;        /* "simpleweighting" (default true) */
+} PbrtRealisticLens;
+/* pbrt_gpu_scene_create_camera with a realistic camera: camera->kind must be PBRT_CAMERA_REALISTIC when lens != NULL; lens == NULL
+ * is pbrt_gpu_scene_create_camera.  Errors as for that call, and: a lens with another kind, n_elements == 0, a null array, a field
+ * that is not finite, a zero full_resolution, a diagonal <= 0 or bounds with pmin > pmax: PBRT_E_INVALID; more than
+ * PBRT_MAX_LENS_ELEMENTS elements: PBRT_E_UNSUPPORTED.  The library keeps no pointer into *lens. */
+int pbrt_gpu_scene_create_lens(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const PbrtRealisticLens* lens,
+                               const int* devices, uint32_t n_devices, PbrtScene** out);
 void pbrt_gpu_scene_destroy(PbrtScene* scene);
 /* Optional (ABI v4): page-lock a host array the caller owns -- nodes, tris, a mesh's p / n / s / uv -- so that pbrt_gpu_scene_create
  * DMAs it where it lies (cudaHostRegister, portable across devices); an array that is not pinned is copied through the library's
@@ -487,6 +534,12 @@ int pbrt_gpu_kat_log2(int device, uint32_t n, const float* x, float* log2_out);
 /* Known-answer hook for motion blur: AnimatedTransform::new of *at on the host, then AnimatedTransform::interpolate on the device at
  * n times, writing 16 floats of m and 16 of m_inv per time (row-major).  Not part of the render path. */
 int pbrt_gpu_kat_animated_interpolate(int device, const PbrtAnimatedTransform* at, uint32_t n, const float* times, float* m_out, float* m_inv_out);
+/* Known-answer hook for the realistic camera: the device's generate_ray_differential of a scene from pbrt_gpu_scene_create_lens for n
+ * camera samples (p_film[2n], p_lens[2n], time[n]), through its camera_to_world (animated or not).  Per sample: o[3], d[3], the
+ * weight, and the world-space differentials rx_o / ry_o / rx_d / ry_d [3] before the 1/sqrt(spp) scale.  Where the weight is 0 the
+ * rays are written as zeros.  Not part of the render path. */
+int pbrt_gpu_kat_realistic_rays(PbrtScene* scene, uint32_t n, const float* p_film, const float* p_lens, const float* time, float* o, float* d,
+                                float* weight, float* rx_o, float* ry_o, float* rx_d, float* ry_d);
 
 #ifdef __cplusplus
 }

@@ -111,6 +111,16 @@ int pbrt_host_camera_orthographic(PbrtHost* h, float lens_radius, float focal_di
 /* Camera "environment" (EnvironmentCamera::create, src/cameras/environment.rs:44-90): camera_to_world, the shutter and the film's
  * full resolution; it reads no screen window and no lens.  Call after pbrt_host_film. */
 int pbrt_host_camera_environment(PbrtHost* h, float shutter_open, float shutter_close);
+/* Film "diagonal" in millimetres (film.rs:250, default 35): the realistic camera's film size.  Call before the camera. */
+int pbrt_host_film_diagonal(PbrtHost* h, float mm);
+/* Camera "realistic" (RealisticCamera::create / new, src/cameras/realistic.rs:50-197): lens_mm holds the lens file's n_values
+ * numbers, rows {radius, thickness, eta, diameter} in mm.  The stop's diameter is replaced by aperture_diameter unless that is
+ * larger; the last thickness is set by focus_thick_lens; the 64 exit-pupil bins are bounded on host threads.  focus_binary_search
+ * is not restated: the reference discards its result.  Where the reference asserts or panics (no ray through the thick-lens
+ * approximation, a focus distance too short) and for a row count that is not a positive multiple of four: PBRT_E_INVALID.
+ * Call after pbrt_host_film (and pbrt_host_film_diagonal). */
+int pbrt_host_camera_realistic(PbrtHost* h, const float* lens_mm, int n_values, float aperture_diameter, float focus_distance, int simple_weighting,
+                               float shutter_open, float shutter_close);
 int pbrt_host_sampler_sobol(PbrtHost* h, int pixel_samples);
 /* Sampler "halton" (src/samplers/halton.rs:162-172), the reference's default sampler; any pixel_samples >= 1. */
 int pbrt_host_sampler_halton(PbrtHost* h, int pixel_samples, int sample_at_pixel_center);
@@ -132,6 +142,12 @@ const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h);
 const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h);
 /* The camera model of the built scene (its kind and Film.full_resolution) for pbrt_gpu_scene_create_camera. */
 const PbrtCameraModel* pbrt_host_camera_model(const PbrtHost* h);
+/* RealisticCamera::bound_exit_pupil of the 64 film-radius bins (realistic.rs:100-139,573-652) for a lens given in metres, film
+ * side last, whose last thickness is already the lens-film distance: 64 x {pmin.x, pmin.y, pmax.x, pmax.y}.  What
+ * pbrt_host_camera_realistic computes after focusing. */
+int pbrt_host_lens_exit_pupil(const PbrtLensElement* elements, int n_elements, float film_diagonal_m, float* bounds);
+/* The realistic camera of the built scene for pbrt_gpu_scene_create_lens; NULL for any other camera. */
+const PbrtRealisticLens* pbrt_host_lens(const PbrtHost* h);
 
 /* Integrator::render(scene, num_threads): uploads the scene, renders pixel_rect (NULL = whole sample bounds) on `device`
  * through pbrt_gpu_render, and merges the result into the Film like merge_film_tile. */

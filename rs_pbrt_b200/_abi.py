@@ -85,10 +85,21 @@ class PbrtMotionDesc(C.Structure):
 
 
 PBRT_CAMERA_PERSPECTIVE, PBRT_CAMERA_ORTHOGRAPHIC, PBRT_CAMERA_ENVIRONMENT = 0, 1, 2
+PBRT_CAMERA_REALISTIC = 3
+PBRT_MAX_LENS_ELEMENTS = 32
 
 
 class PbrtCameraModel(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("full_resolution", C.c_uint32 * 2)]
+
+
+class PbrtLensElement(C.Structure):
+    _fields_ = [("curvature_radius", C.c_float), ("thickness", C.c_float), ("eta", C.c_float), ("aperture_radius", C.c_float)]
+
+
+class PbrtRealisticLens(C.Structure):
+    _fields_ = [("elements", C.POINTER(PbrtLensElement)), ("n_elements", C.c_uint32), ("exit_pupil_bounds", C.POINTER(C.c_float)),
+                ("film_diagonal", C.c_float), ("simple_weighting", C.c_uint32)]
 
 
 class PbrtRenderParams(C.Structure):
@@ -112,9 +123,10 @@ class PbrtStats(C.Structure):
 GPU_SYMBOLS = ["pbrt_gpu_scene_create", "pbrt_gpu_scene_destroy", "pbrt_gpu_scene_bytes", "pbrt_gpu_render", "pbrt_gpu_render_device", "pbrt_gpu_render_samples",
                "pbrt_gpu_render_tiles_device", "pbrt_gpu_render_multi", "pbrt_gpu_host_register", "pbrt_gpu_host_unregister",
                "pbrt_gpu_intersect", "pbrt_gpu_intersect_p", "pbrt_gpu_last_error", "pbrt_gpu_abi_version", "pbrt_gpu_launch_count", "pbrt_gpu_kat_sincos", "pbrt_gpu_kat_acos_atan2", "pbrt_gpu_kat_log2",
-               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate", "pbrt_gpu_scene_create_multi", "pbrt_gpu_scene_create_camera"]
+               "pbrt_gpu_scene_create_motion", "pbrt_gpu_kat_animated_interpolate", "pbrt_gpu_scene_create_multi", "pbrt_gpu_scene_create_camera",
+               "pbrt_gpu_scene_create_lens", "pbrt_gpu_kat_realistic_rays"]
 HOST_SYMBOLS = ["pbrt_host_new", "pbrt_host_free", "pbrt_host_last_error", "pbrt_host_add_material", "pbrt_host_add_material_mix", "pbrt_host_add_trianglemesh",
-                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_camera_orthographic", "pbrt_host_camera_environment", "pbrt_host_camera_model", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
+                "pbrt_host_add_light_point", "pbrt_host_add_light_spot", "pbrt_host_add_light_distant", "pbrt_host_add_light_infinite", "pbrt_host_add_light_goniometric", "pbrt_host_add_light_projection", "pbrt_host_look_at", "pbrt_host_transform_times", "pbrt_host_camera_motion", "pbrt_host_motion_desc", "pbrt_host_film", "pbrt_host_camera_perspective", "pbrt_host_camera_orthographic", "pbrt_host_camera_environment", "pbrt_host_camera_model", "pbrt_host_camera_realistic", "pbrt_host_film_diagonal", "pbrt_host_lens", "pbrt_host_lens_exit_pupil", "pbrt_host_sampler_sobol", "pbrt_host_sampler_halton", "pbrt_host_integrator_ao", "pbrt_host_object_begin", "pbrt_host_object_end", "pbrt_host_object_instance", "pbrt_host_instancing", "pbrt_host_add_texture_image", "pbrt_host_material_texture", "pbrt_host_material_bump", "pbrt_host_mesh_alpha", "pbrt_host_texture_mapping", "pbrt_host_add_texture_constant", "pbrt_host_add_texture_scale", "pbrt_host_add_texture_mix", "pbrt_host_integrator_direct", "pbrt_host_integrator_whitted", "pbrt_host_light_samples",
                 "pbrt_host_integrator_path", "pbrt_host_world_end", "pbrt_host_scene_desc", "pbrt_host_render_params", "pbrt_host_render",
                 "pbrt_host_film_rgbw", "pbrt_host_film_clear", "pbrt_host_film_add_rgbw", "pbrt_host_film_rgb", "pbrt_host_write_image",
                 "pbrt_host_bvh_build"]
@@ -146,6 +158,9 @@ def bind(L):
     L.pbrt_gpu_scene_create_multi.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(C.c_int), C.c_uint32, C.POINTER(vp)]
     L.pbrt_gpu_scene_create_camera.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(PbrtCameraModel), C.POINTER(C.c_int), C.c_uint32,
                                                C.POINTER(vp)]
+    L.pbrt_gpu_scene_create_lens.argtypes = [C.POINTER(PbrtSceneDesc), C.POINTER(PbrtMotionDesc), C.POINTER(PbrtCameraModel), C.POINTER(PbrtRealisticLens),
+                                             C.POINTER(C.c_int), C.c_uint32, C.POINTER(vp)]
+    L.pbrt_gpu_kat_realistic_rays.argtypes = [vp, C.c_uint32, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp]
     L.pbrt_gpu_kat_animated_interpolate.argtypes = [C.c_int, C.POINTER(PbrtAnimatedTransform), C.c_uint32, fp, fp, fp]
     L.pbrt_gpu_scene_destroy.argtypes = [vp]
     L.pbrt_gpu_scene_destroy.restype = None
@@ -189,6 +204,11 @@ def bind(L):
     L.pbrt_host_camera_environment.argtypes = [vp, C.c_float, C.c_float]
     L.pbrt_host_camera_model.argtypes = [vp]
     L.pbrt_host_camera_model.restype = C.POINTER(PbrtCameraModel)
+    L.pbrt_host_camera_realistic.argtypes = [vp, fp, C.c_int, C.c_float, C.c_float, C.c_int, C.c_float, C.c_float]
+    L.pbrt_host_film_diagonal.argtypes = [vp, C.c_float]
+    L.pbrt_host_lens.argtypes = [vp]
+    L.pbrt_host_lens_exit_pupil.argtypes = [C.POINTER(PbrtLensElement), C.c_int, C.c_float, fp]
+    L.pbrt_host_lens.restype = C.POINTER(PbrtRealisticLens)
     L.pbrt_host_sampler_sobol.argtypes = [vp, C.c_int]
     L.pbrt_host_sampler_halton.argtypes = [vp, C.c_int, C.c_int]
     L.pbrt_host_integrator_ao.argtypes = [vp, C.c_int, C.c_int]

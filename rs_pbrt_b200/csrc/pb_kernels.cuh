@@ -19,6 +19,7 @@
 #include "pb_texture.cuh"
 #include "pb_material.cuh"
 #include "pb_motion.cuh"
+#include "pb_lens.cuh"
 
 namespace pb {
 
@@ -99,17 +100,57 @@ struct BatchInfo {
     uint32_t n_samples;
 };
 
+// k_raygen's slot for the realistic camera (integrator.rs:134-160): the camera sample's ray and weight.  A vignetted sample (weight 0)
+// keeps a valid p_film and no PF_HAS_RAY: li does not run (L = 0), and k_resolve<true> still adds its filter weight to the pixel.
+template <bool CAM_MOTION>
+PB_D uint32_t raygen_lens(const DScene& sc, const DRender& rp, DPaths& ps, const DLens& lens, const DMotion& cam_mo, uint32_t i, uint64_t index, float2 p_film,
+                          float time, float2 p_lens, float4& ray0, float4& ray1) {
+    float c2w_t[16];
+    if (CAM_MOTION) {
+        float c2w_inv_t[16];
+        motion_interpolate(cam_mo, lerpf(time, sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
+    }
+    const float* c = CAM_MOTION ? c2w_t : sc.camera_to_world;
+    V3 o, d, rxo, ryo, rxd, ryd;
+    const float wt = lens_generate_ray_differential(lens, c, make_float2(sc.shutter_open, sc.shutter_close), p_film, p_lens, o, d, rxo, ryo, rxd, ryd);
+    lens.weight[i] = wt;
+    ps.p_film[i] = p_film;
+    if (!(wt > 0.0f)) {  // integrator.rs:157: li only for ray_weight > 0
+        ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0u));
+        return 0;
+    }
+    if (ps.ray_diff) {  // scale_differentials(1 / sqrt(spp)) (integrator.rs:140-144)
+        const float sdiff = 1.0f / sqrtf((float)rp.spp);
+        rxo = o + (rxo - o) * sdiff;
+        ryo = o + (ryo - o) * sdiff;
+        rxd = d + (rxd - d) * sdiff;
+        ryd = d + (ryd - d) * sdiff;
+        ps.ray_diff[3 * (size_t)i] = make_float4(rxo.x, rxo.y, rxo.z, ryo.x);
+        ps.ray_diff[3 * (size_t)i + 1] = make_float4(ryo.y, ryo.z, rxd.x, rxd.y);
+        ps.ray_diff[3 * (size_t)i + 2] = make_float4(rxd.z, ryd.x, ryd.y, ryd.z);
+    }
+    ps.ray_d[i] = make_float4(d.x, d.y, d.z, 0.0f);
+    ray0 = make_float4(o.x, o.y, o.z, __int_as_float(0x7f800000));
+    ray1 = make_float4(d.x, d.y, d.z, __uint_as_float(i | (RAY_EXTEND << 30)));
+    ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+    ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(PF_HAS_RAY));
+    ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
+    ps.dim[i] = 5u;
+    return 1;
+}
+
 // -----------------------------------------------------------------------------------------------
 // k_raygen: integrator.rs:123-144, sampler.rs:85-95, sobol.rs:110-138, and the camera's generate_ray_differential
 // (perspective.rs:190-280, orthographic.rs:156-230, environment.rs:92-116).
 // CAM_MOTION: the camera is animated (cam_mo); a static camera's instantiation never reads cam_mo.
-// CAM_KIND: PbrtCameraKind.  env_res: Film.full_resolution as floats, read by the environment camera only.
+// CAM_KIND: PbrtCameraKind.  env_res: Film.full_resolution as floats, read by the environment camera only.  lens: the realistic
+// camera's lens system, pupil bounds and per-slot weight array, read by that camera only.
 template <bool CAM_MOTION, int CAM_KIND>
 __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps, BatchInfo bi, const uint32_t* __restrict__ nib, uint32_t n_chunks,
                                                const uint64_t* __restrict__ vdc, const uint64_t* __restrict__ vdci, uint32_t* __restrict__ queue,
                                                uint32_t* __restrict__ d_count, float4* __restrict__ rays, uint32_t* __restrict__ d_nrays,
-                                               DCounters* cnt, const DMotion cam_mo, const float2 env_res) {
-    constexpr bool ORTHO = CAM_KIND == PBRT_CAMERA_ORTHOGRAPHIC, ENV = CAM_KIND == PBRT_CAMERA_ENVIRONMENT;
+                                               DCounters* cnt, const DMotion cam_mo, const float2 env_res, const DLens lens) {
+    constexpr bool ORTHO = CAM_KIND == PBRT_CAMERA_ORTHOGRAPHIC, ENV = CAM_KIND == PBRT_CAMERA_ENVIRONMENT, REAL = CAM_KIND == PBRT_CAMERA_REALISTIC;
     __shared__ uint64_t s_vdc[52], s_vdci[52];
     if (threadIdx.x < 52) {
         uint32_t m = rp.log2_res;
@@ -158,109 +199,113 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
                 lx = sobol_sample_nib(sob, 3);
             }
             float2 p_film = make_float2((float)px + sx, (float)py + sy);
-            // raster -> camera (Transform::transform_point transform.rs:490-517)
-            const float* m = sc.raster_to_camera;
-            float x = p_film.x, y = p_film.y, z = 0.0f;
-            float xp = m[0] * x + m[1] * y + m[2] * z + m[3];
-            float yp = m[4] * x + m[5] * y + m[6] * z + m[7];
-            float zp = m[8] * x + m[9] * y + m[10] * z + m[11];
-            float wp = m[12] * x + m[13] * y + m[14] * z + m[15];
-            V3 pc = mk3(xp, yp, zp);
-            if (wp != 1.0f) { float inv = 1.0f / wp; pc = mk3(inv * xp, inv * yp, inv * zp); }
-            V3 o = mk3(0.0f, 0.0f, 0.0f), d = norm3(pc);
-            if (ORTHO) { o = pc; d = mk3(0.0f, 0.0f, 1.0f); }  // orthographic.rs:165-176
-            if (ENV) {  // environment.rs:93-100 (f32 sin / cos: the glibc restatement)
-                const float theta = PB_PI * p_film.y / env_res.y, phi = 2.0f * PB_PI * p_film.x / env_res.x;
-                float st, ct, sp, cp;
-                sincos_rn(theta, st, ct);
-                sincos_rn(phi, sp, cp);
-                d = mk3(st * cp, ct, st * sp);
-            }
-            (void)time;  // ray.time only selects an animated transform; static cameras ignore it
-            float c2w_t[16];
-            if (CAM_MOTION) {  // AnimatedTransform::transform_ray (transform.rs:2114-2124) at ray.time = lerp(sample.time, shutter) (perspective.rs:226)
-                float c2w_inv_t[16];
-                motion_interpolate(cam_mo, lerpf(time, sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
-            }
-            if (!ENV && sc.lens_radius > 0.0f) {  // (the same thin lens for the orthographic camera, orthographic.rs:177-188)
-                float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
-                pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
-                float ft = sc.focal_distance / d.z;
-                V3 p_focus = o + d * ft;
-                o = mk3(pl2.x, pl2.y, 0.0f);
-                d = norm3(p_focus - o);
-            }
-            // camera -> world (Transform::transform_ray transform.rs:538-550, with origin error offset :662-708)
-            const float* c = CAM_MOTION ? c2w_t : sc.camera_to_world;
-            x = o.x; y = o.y; z = o.z;
-            V3 ow = mk3(c[0] * x + c[1] * y + c[2] * z + c[3], c[4] * x + c[5] * y + c[6] * z + c[7], c[8] * x + c[9] * y + c[10] * z + c[11]);
-            float wpc = c[12] * x + c[13] * y + c[14] * z + c[15];
-            V3 o_err = mk3(fabsf(c[0] * x) + fabsf(c[1] * y) + fabsf(c[2] * z) + fabsf(c[3]), fabsf(c[4] * x) + fabsf(c[5] * y) + fabsf(c[6] * z) + fabsf(c[7]),
-                           fabsf(c[8] * x) + fabsf(c[9] * y) + fabsf(c[10] * z) + fabsf(c[11])) * gamma_n(3);
-            if (wpc != 1.0f) { float inv = 1.0f / wpc; ow = mk3(inv * ow.x, inv * ow.y, inv * ow.z); }
-            V3 dw = mk3(c[0] * d.x + c[1] * d.y + c[2] * d.z, c[4] * d.x + c[5] * d.y + c[6] * d.z, c[8] * d.x + c[9] * d.y + c[10] * d.z);
-            float ls = len2(dw);
-            if (ls > 0.0f) {
-                float dt = dot3(abs3(dw), o_err) / ls;
-                ow = ow + dw * dt;
-            }
-            // textured scenes: the ray differential (perspective.rs:205-271), through camera_to_world (transform.rs:550-556), scaled
-            // (integrator.rs:140-144).  The environment camera makes none (environment.rs:106).
-            if (!ENV && ps.ray_diff) {
-                const V3 dxc = mk3(sc.dx_camera[0], sc.dx_camera[1], sc.dx_camera[2]), dyc = mk3(sc.dy_camera[0], sc.dy_camera[1], sc.dy_camera[2]);
-                V3 rxo = mk3(0.0f, 0.0f, 0.0f), ryo = rxo;
-                V3 rxd = norm3(pc + dxc), ryd = norm3(pc + dyc);
-                if (ORTHO) {  // orthographic.rs:189-226
-                    rxo = o + dxc; ryo = o + dyc; rxd = d; ryd = d;
-                    if (sc.lens_radius > 0.0f) {
-                        // ft of the refracted ray.d, and one focus point (from dx_camera) for both differentials: ry == rx, as written
-                        float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
-                        pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
-                        const float ft = sc.focal_distance / d.z;
-                        const V3 p_focus = pc + dxc + mk3(0.0f, 0.0f, 1.0f) * ft;
-                        rxo = mk3(pl2.x, pl2.y, 0.0f); ryo = rxo;
-                        rxd = norm3(p_focus - rxo); ryd = norm3(p_focus - ryo);
-                    }
-                } else if (sc.lens_radius > 0.0f) {
+            if constexpr (REAL) {  // realistic.rs:693-735 (pb_lens.cuh)
+                my_rays = raygen_lens<CAM_MOTION>(sc, rp, ps, lens, cam_mo, i, index, p_film, time, make_float2(lx, ly), ray0, ray1);
+            } else {
+                // raster -> camera (Transform::transform_point transform.rs:490-517)
+                const float* m = sc.raster_to_camera;
+                float x = p_film.x, y = p_film.y, z = 0.0f;
+                float xp = m[0] * x + m[1] * y + m[2] * z + m[3];
+                float yp = m[4] * x + m[5] * y + m[6] * z + m[7];
+                float zp = m[8] * x + m[9] * y + m[10] * z + m[11];
+                float wp = m[12] * x + m[13] * y + m[14] * z + m[15];
+                V3 pc = mk3(xp, yp, zp);
+                if (wp != 1.0f) { float inv = 1.0f / wp; pc = mk3(inv * xp, inv * yp, inv * zp); }
+                V3 o = mk3(0.0f, 0.0f, 0.0f), d = norm3(pc);
+                if (ORTHO) { o = pc; d = mk3(0.0f, 0.0f, 1.0f); }  // orthographic.rs:165-176
+                if (ENV) {  // environment.rs:93-100 (f32 sin / cos: the glibc restatement)
+                    const float theta = PB_PI * p_film.y / env_res.y, phi = 2.0f * PB_PI * p_film.x / env_res.x;
+                    float st, ct, sp, cp;
+                    sincos_rn(theta, st, ct);
+                    sincos_rn(phi, sp, cp);
+                    d = mk3(st * cp, ct, st * sp);
+                }
+                (void)time;  // ray.time only selects an animated transform; static cameras ignore it
+                float c2w_t[16];
+                if (CAM_MOTION) {  // AnimatedTransform::transform_ray (transform.rs:2114-2124) at ray.time = lerp(sample.time, shutter) (perspective.rs:226)
+                    float c2w_inv_t[16];
+                    motion_interpolate(cam_mo, lerpf(time, sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
+                }
+                if (!ENV && sc.lens_radius > 0.0f) {  // (the same thin lens for the orthographic camera, orthographic.rs:177-188)
                     float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
                     pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
-                    const V3 dx = norm3(pc + dxc);
-                    const float ftx = sc.focal_distance / dx.z;
-                    const V3 pfx = mk3(0.0f, 0.0f, 0.0f) + dx * ftx;
-                    rxo = mk3(pl2.x, pl2.y, 0.0f);
-                    rxd = norm3(pfx - rxo);
-                    const V3 dy = norm3(pc + dyc);
-                    const float fty = sc.focal_distance / dy.z;
-                    const V3 pfy = mk3(0.0f, 0.0f, 0.0f) + dy * fty;
-                    ryo = mk3(pl2.x, pl2.y, 0.0f);
-                    ryd = norm3(pfy - ryo);
+                    float ft = sc.focal_distance / d.z;
+                    V3 p_focus = o + d * ft;
+                    o = mk3(pl2.x, pl2.y, 0.0f);
+                    d = norm3(p_focus - o);
                 }
-                auto xp = [c](V3 q) {
-                    V3 r = mk3(c[0] * q.x + c[1] * q.y + c[2] * q.z + c[3], c[4] * q.x + c[5] * q.y + c[6] * q.z + c[7], c[8] * q.x + c[9] * q.y + c[10] * q.z + c[11]);
-                    const float w = c[12] * q.x + c[13] * q.y + c[14] * q.z + c[15];
-                    if (w != 1.0f) { const float inv = 1.0f / w; r = mk3(inv * r.x, inv * r.y, inv * r.z); }
-                    return r;
-                };
-                auto xv = [c](V3 v) { return mk3(c[0] * v.x + c[1] * v.y + c[2] * v.z, c[4] * v.x + c[5] * v.y + c[6] * v.z, c[8] * v.x + c[9] * v.y + c[10] * v.z); };
-                rxo = xp(rxo); ryo = xp(ryo); rxd = xv(rxd); ryd = xv(ryd);
-                const float sdiff = 1.0f / sqrtf((float)rp.spp);
-                rxo = ow + (rxo - ow) * sdiff;
-                ryo = ow + (ryo - ow) * sdiff;
-                rxd = dw + (rxd - dw) * sdiff;
-                ryd = dw + (ryd - dw) * sdiff;
-                ps.ray_diff[3 * (size_t)i] = make_float4(rxo.x, rxo.y, rxo.z, ryo.x);
-                ps.ray_diff[3 * (size_t)i + 1] = make_float4(ryo.y, ryo.z, rxd.x, rxd.y);
-                ps.ray_diff[3 * (size_t)i + 2] = make_float4(rxd.z, ryd.x, ryd.y, ryd.z);
+                // camera -> world (Transform::transform_ray transform.rs:538-550, with origin error offset :662-708)
+                const float* c = CAM_MOTION ? c2w_t : sc.camera_to_world;
+                x = o.x; y = o.y; z = o.z;
+                V3 ow = mk3(c[0] * x + c[1] * y + c[2] * z + c[3], c[4] * x + c[5] * y + c[6] * z + c[7], c[8] * x + c[9] * y + c[10] * z + c[11]);
+                float wpc = c[12] * x + c[13] * y + c[14] * z + c[15];
+                V3 o_err = mk3(fabsf(c[0] * x) + fabsf(c[1] * y) + fabsf(c[2] * z) + fabsf(c[3]), fabsf(c[4] * x) + fabsf(c[5] * y) + fabsf(c[6] * z) + fabsf(c[7]),
+                               fabsf(c[8] * x) + fabsf(c[9] * y) + fabsf(c[10] * z) + fabsf(c[11])) * gamma_n(3);
+                if (wpc != 1.0f) { float inv = 1.0f / wpc; ow = mk3(inv * ow.x, inv * ow.y, inv * ow.z); }
+                V3 dw = mk3(c[0] * d.x + c[1] * d.y + c[2] * d.z, c[4] * d.x + c[5] * d.y + c[6] * d.z, c[8] * d.x + c[9] * d.y + c[10] * d.z);
+                float ls = len2(dw);
+                if (ls > 0.0f) {
+                    float dt = dot3(abs3(dw), o_err) / ls;
+                    ow = ow + dw * dt;
+                }
+                // textured scenes: the ray differential (perspective.rs:205-271), through camera_to_world (transform.rs:550-556), scaled
+                // (integrator.rs:140-144).  The environment camera makes none (environment.rs:106).
+                if (!ENV && ps.ray_diff) {
+                    const V3 dxc = mk3(sc.dx_camera[0], sc.dx_camera[1], sc.dx_camera[2]), dyc = mk3(sc.dy_camera[0], sc.dy_camera[1], sc.dy_camera[2]);
+                    V3 rxo = mk3(0.0f, 0.0f, 0.0f), ryo = rxo;
+                    V3 rxd = norm3(pc + dxc), ryd = norm3(pc + dyc);
+                    if (ORTHO) {  // orthographic.rs:189-226
+                        rxo = o + dxc; ryo = o + dyc; rxd = d; ryd = d;
+                        if (sc.lens_radius > 0.0f) {
+                            // ft of the refracted ray.d, and one focus point (from dx_camera) for both differentials: ry == rx, as written
+                            float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
+                            pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
+                            const float ft = sc.focal_distance / d.z;
+                            const V3 p_focus = pc + dxc + mk3(0.0f, 0.0f, 1.0f) * ft;
+                            rxo = mk3(pl2.x, pl2.y, 0.0f); ryo = rxo;
+                            rxd = norm3(p_focus - rxo); ryd = norm3(p_focus - ryo);
+                        }
+                    } else if (sc.lens_radius > 0.0f) {
+                        float2 pl2 = concentric_sample_disk(make_float2(lx, ly));
+                        pl2 = make_float2(pl2.x * sc.lens_radius, pl2.y * sc.lens_radius);
+                        const V3 dx = norm3(pc + dxc);
+                        const float ftx = sc.focal_distance / dx.z;
+                        const V3 pfx = mk3(0.0f, 0.0f, 0.0f) + dx * ftx;
+                        rxo = mk3(pl2.x, pl2.y, 0.0f);
+                        rxd = norm3(pfx - rxo);
+                        const V3 dy = norm3(pc + dyc);
+                        const float fty = sc.focal_distance / dy.z;
+                        const V3 pfy = mk3(0.0f, 0.0f, 0.0f) + dy * fty;
+                        ryo = mk3(pl2.x, pl2.y, 0.0f);
+                        ryd = norm3(pfy - ryo);
+                    }
+                    auto xp = [c](V3 q) {
+                        V3 r = mk3(c[0] * q.x + c[1] * q.y + c[2] * q.z + c[3], c[4] * q.x + c[5] * q.y + c[6] * q.z + c[7], c[8] * q.x + c[9] * q.y + c[10] * q.z + c[11]);
+                        const float w = c[12] * q.x + c[13] * q.y + c[14] * q.z + c[15];
+                        if (w != 1.0f) { const float inv = 1.0f / w; r = mk3(inv * r.x, inv * r.y, inv * r.z); }
+                        return r;
+                    };
+                    auto xv = [c](V3 v) { return mk3(c[0] * v.x + c[1] * v.y + c[2] * v.z, c[4] * v.x + c[5] * v.y + c[6] * v.z, c[8] * v.x + c[9] * v.y + c[10] * v.z); };
+                    rxo = xp(rxo); ryo = xp(ryo); rxd = xv(rxd); ryd = xv(ryd);
+                    const float sdiff = 1.0f / sqrtf((float)rp.spp);
+                    rxo = ow + (rxo - ow) * sdiff;
+                    ryo = ow + (ryo - ow) * sdiff;
+                    rxd = dw + (rxd - dw) * sdiff;
+                    ryd = dw + (ryd - dw) * sdiff;
+                    ps.ray_diff[3 * (size_t)i] = make_float4(rxo.x, rxo.y, rxo.z, ryo.x);
+                    ps.ray_diff[3 * (size_t)i + 1] = make_float4(ryo.y, ryo.z, rxd.x, rxd.y);
+                    ps.ray_diff[3 * (size_t)i + 2] = make_float4(rxd.z, ryd.x, ryd.y, ryd.z);
+                }
+                ps.ray_d[i] = make_float4(dw.x, dw.y, dw.z, 0.0f);
+                ray0 = make_float4(ow.x, ow.y, ow.z, __int_as_float(0x7f800000));  // t_max = inf - dt = inf
+                ray1 = make_float4(dw.x, dw.y, dw.z, __uint_as_float(i | (RAY_EXTEND << 30)));
+                ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+                ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(PF_HAS_RAY));
+                ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
+                ps.dim[i] = 5u;
+                ps.p_film[i] = p_film;
+                my_rays = 1;
             }
-            ps.ray_d[i] = make_float4(dw.x, dw.y, dw.z, 0.0f);
-            ray0 = make_float4(ow.x, ow.y, ow.z, __int_as_float(0x7f800000));  // t_max = inf - dt = inf
-            ray1 = make_float4(dw.x, dw.y, dw.z, __uint_as_float(i | (RAY_EXTEND << 30)));
-            ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
-            ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(PF_HAS_RAY));
-            ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
-            ps.dim[i] = 5u;
-            ps.p_film[i] = p_film;
-            my_rays = 1;
         }
     }
     uint32_t pos = queue_append(d_nrays, my_rays != 0);  // *d_nrays is zeroed by the host before the launch
@@ -1238,6 +1283,27 @@ __global__ void k_kat_motion(const DMotion mo, const float* __restrict__ t, uint
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) motion_interpolate(mo, t[i], m + 16 * (size_t)i, m_inv + 16 * (size_t)i);
 }
+// known-answer hook for the realistic camera's generate_ray_differential (pbrt_gpu_kat_realistic_rays): in[i] = {p_film, p_lens},
+// time[i]; out: 19 floats per sample, o[3] d[3] weight rx_o[3] ry_o[3] rx_d[3] ry_d[3], zeros where the weight is 0
+__global__ void k_kat_realistic(const DScene sc, const DLens lens, const DMotion cam_mo, uint32_t cam_motion, const float4* __restrict__ in,
+                                const float* __restrict__ time, uint32_t n, float* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float c2w_t[16], c2w_inv_t[16];
+    if (cam_motion) motion_interpolate(cam_mo, lerpf(time[i], sc.shutter_open, sc.shutter_close), c2w_t, c2w_inv_t);
+    const float4 q = in[i];
+    V3 o, d, rxo, ryo, rxd, ryd;
+    const float wt = lens_generate_ray_differential(lens, cam_motion ? c2w_t : sc.camera_to_world, make_float2(sc.shutter_open, sc.shutter_close),
+                                                    make_float2(q.x, q.y), make_float2(q.z, q.w), o, d, rxo, ryo, rxd, ryd);
+    float* r = out + 19 * (size_t)i;
+    const V3 v[6] = {o, d, rxo, ryo, rxd, ryd};
+    for (int k = 0; k < 6; ++k) {
+        r[(k < 2 ? 3 * k : 3 * k + 1)] = wt != 0.0f ? v[k].x : 0.0f;
+        r[(k < 2 ? 3 * k : 3 * k + 1) + 1] = wt != 0.0f ? v[k].y : 0.0f;
+        r[(k < 2 ? 3 * k : 3 * k + 1) + 2] = wt != 0.0f ? v[k].z : 0.0f;
+    }
+    r[6] = wt;
+}
 // known-answer hook for the device sin/cos (pbrt_gpu_kat_sincos)
 __global__ void k_kat_sincos(const float* __restrict__ x, uint32_t n, float* __restrict__ s, float* __restrict__ c) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1264,8 +1330,11 @@ __global__ void k_kat_acos_atan2(const float* __restrict__ x, const float* __res
 // Contributions to the sample's own pixel are summed in registers in the reference's order; the
 // rare contributions to neighbouring pixels (filter footprint, sobol.rs:132-137 apron case) use
 // atomics, like the unordered tile merge of the reference (integrator.rs:209-215).
+// WEIGHTED: the realistic camera's ray weights (k_raygen's DLens.weight), multiplied in the reference's order L * weight * filter
+// weight; every other camera's weight is 1 and its instantiation never reads `weight`.
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(256) k_resolve(DRender rp, DPaths ps, BatchInfo bi, const float* __restrict__ filter_table, float* __restrict__ film,
-                                                float* __restrict__ sample_rgb) {
+                                                float* __restrict__ sample_rgb, const float* __restrict__ weight) {
     uint32_t pl = blockIdx.x * blockDim.x + threadIdx.x;
     if (pl >= bi.n_pixels) return;
     uint32_t pix = bi.first_pixel + pl;
@@ -1297,7 +1366,7 @@ __global__ void __launch_bounds__(256) k_resolve(DRender rp, DPaths ps, BatchInf
                 float fx = fabsf(((float)x - dx) * inv_rx * 16.0f);
                 int ix = f2i_sat(fminf(floorf(fx), 15.0f));
                 float w = __ldg(filter_table + iy * 16 + ix);
-                Sp c = l * sp1(1.0f) * sp1(w);  // sample_weight = 1 (perspective camera)
+                Sp c = l * sp1(WEIGHTED ? weight[slot] : 1.0f) * sp1(w);  // sample_weight = 1 but for the realistic camera
                 if (x == px && y == py) { ar += c.r; ag += c.g; ab += c.b; aw += w; }
                 else {
                     float* d = film + 4 * ((size_t)(y - rp.cb[1]) * fw + (x - rp.cb[0]));

@@ -449,6 +449,7 @@ struct BatchCtx {
     DevBuf<uint32_t> occl, cls_queue, queue[2], counts, dim;
     DevBuf<uint2> sobol;
     DevBuf<float2> pfilm;
+    DevBuf<float> cam_weight;                       // realistic camera: per-slot camera ray weight (k_raygen -> k_resolve<true>)
     DevBuf<int> g_state;
     DevBuf<float> g_func, g_cdf, g_fint, g_contrib;
     DevBuf<uint32_t> g_request;
@@ -569,6 +570,7 @@ struct PbrtScene {
     DMotion cam_mo;
     uint32_t cam_kind = PBRT_CAMERA_PERSPECTIVE;  // PbrtCameraKind: k_raygen's second template argument
     float2 env_res = {0.0f, 0.0f};                // the environment camera's Film.full_resolution
+    DLens lens = {};                              // the realistic camera's lens (k_raygen's trailing argument; weight set per launch)
     int light_level = 0;  // light level of the kernels that sample lights (pb_interaction.cuh): 0 = area lights only, 1 = any but image lights, 2 = with them
     uint32_t class_mask = 0;  // bit c: some material has shading class c (1..8: a single lobe of kind c - 1; 9: Lambert + microfacet reflection; 10..15: everything else)
     size_t upload_bytes = 0;
@@ -747,8 +749,18 @@ static bool enable_peer_access(int from, int to) {
 static decltype(&k_raygen<false, PBRT_CAMERA_PERSPECTIVE>) raygen_kernel(const PbrtScene* sc) {
     if (sc->cam_kind == PBRT_CAMERA_ORTHOGRAPHIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ORTHOGRAPHIC> : k_raygen<false, PBRT_CAMERA_ORTHOGRAPHIC>;
     if (sc->cam_kind == PBRT_CAMERA_ENVIRONMENT) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ENVIRONMENT> : k_raygen<false, PBRT_CAMERA_ENVIRONMENT>;
+    if (sc->cam_kind == PBRT_CAMERA_REALISTIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_REALISTIC> : k_raygen<false, PBRT_CAMERA_REALISTIC>;
     return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_PERSPECTIVE> : k_raygen<false, PBRT_CAMERA_PERSPECTIVE>;
 }
+
+// k_raygen's lens argument: the scene's realistic-camera record with this batch context's weight array (unused by other cameras)
+static DLens lens_arg(const PbrtScene* sc, const BatchCtx& X) {
+    DLens L = sc->lens;
+    L.weight = X.cam_weight.p;
+    return L;
+}
+// k_resolve's instantiation: the realistic camera's samples carry a weight, every other camera's weight is 1
+static decltype(&k_resolve<false>) resolve_kernel(const PbrtScene* sc) { return sc->cam_kind == PBRT_CAMERA_REALISTIC ? k_resolve<true> : k_resolve<false>; }
 
 // ---- scene creation --------------------------------------------------------------------------------------------------------------
 // pbrt_gpu_scene_create, _create_motion and _create_multi are one code path in two phases.  scene_prepare validates the description
@@ -798,6 +810,7 @@ struct ScenePrep {
     DMotion cam_mo;
     uint32_t cam_kind = PBRT_CAMERA_PERSPECTIVE;
     float2 env_res = {0.0f, 0.0f};
+    DLens lens = {};
 };
 
 // The host-side passes run on all cores (a 4.3 M-triangle scene is re-uploaded on every end-to-end step).
@@ -836,12 +849,51 @@ static int tri_fail(int code) {
     return fail(PBRT_E_INVALID, "instance index out of range");
 }
 
-static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, ScenePrep& P) {
+// The realistic camera's record (pb_lens.cuh) from the caller's lens, validated.
+static int lens_prepare(const PbrtCameraModel* camera, const PbrtRealisticLens* lens, DLens& L) {
+    if (!camera || camera->kind != PBRT_CAMERA_REALISTIC) return fail(PBRT_E_INVALID, "a lens with a camera kind other than PBRT_CAMERA_REALISTIC");
+    if (!lens->elements || !lens->exit_pupil_bounds || lens->n_elements == 0) return fail(PBRT_E_INVALID, "realistic camera without lens elements or pupil bounds");
+    if (lens->n_elements > PBRT_MAX_LENS_ELEMENTS) return fail(PBRT_E_UNSUPPORTED, "more lens elements than PBRT_MAX_LENS_ELEMENTS");
+    if (camera->full_resolution[0] == 0 || camera->full_resolution[1] == 0) return fail(PBRT_E_INVALID, "realistic camera with a zero full_resolution");
+    if (!std::isfinite(lens->film_diagonal) || !(lens->film_diagonal > 0.0f)) return fail(PBRT_E_INVALID, "realistic camera with a film diagonal <= 0");
+    std::memset(&L, 0, sizeof L);
+    for (uint32_t i = 0; i < lens->n_elements; ++i) {
+        const PbrtLensElement& e = lens->elements[i];
+        if (!std::isfinite(e.curvature_radius) || !std::isfinite(e.thickness) || !std::isfinite(e.eta) || !std::isfinite(e.aperture_radius))
+            return fail(PBRT_E_INVALID, "lens element with a field that is not finite");
+        L.el[i] = make_float4(e.curvature_radius, e.thickness, e.eta, e.aperture_radius);
+    }
+    for (int b = 0; b < PB_PUPIL_BINS; ++b) {
+        const float* q = lens->exit_pupil_bounds + 4 * b;
+        for (int k = 0; k < 4; ++k)
+            if (!std::isfinite(q[k])) return fail(PBRT_E_INVALID, "exit pupil bounds that are not finite");
+        if (q[0] > q[2] || q[1] > q[3]) return fail(PBRT_E_INVALID, "exit pupil bounds with pmin > pmax");
+        L.pupil[b] = make_float4(q[0], q[1], q[2], q[3]);
+    }
+    L.n_el = lens->n_elements;
+    L.simple = lens->simple_weighting ? 1u : 0u;
+    L.diag = lens->film_diagonal;
+    L.full_res = make_float2((float)camera->full_resolution[0], (float)camera->full_resolution[1]);
+    // Film::get_physical_extent (film.rs:293-307), in its f32 order
+    const float aspect = L.full_res.y / L.full_res.x;
+    const float x = std::sqrt(L.diag * L.diag / (1.0f + aspect * aspect)), y = aspect * x;
+    L.ext_min = make_float2(-x / 2.0f, -y / 2.0f);
+    L.ext_max = make_float2(x / 2.0f, y / 2.0f);
+    L.area0 = (L.pupil[0].z - L.pupil[0].x) * (L.pupil[0].w - L.pupil[0].y);  // Bounds2f::area (geometry.rs:1881-1884)
+    return PBRT_OK;
+}
+
+static int scene_prepare(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const PbrtRealisticLens* lens,
+                         ScenePrep& P) {
     P.desc = desc;
     std::memset(&P.cam_mo, 0, sizeof P.cam_mo);
-    if (camera) {
+    if (lens) {
+        const int rc = lens_prepare(camera, lens, P.lens);
+        if (rc != PBRT_OK) return rc;
+        P.cam_kind = PBRT_CAMERA_REALISTIC;
+    } else if (camera) {
         if (camera->kind != PBRT_CAMERA_PERSPECTIVE && camera->kind != PBRT_CAMERA_ORTHOGRAPHIC && camera->kind != PBRT_CAMERA_ENVIRONMENT)
-            return fail(PBRT_E_UNSUPPORTED, "camera kind outside the GPU path (perspective, orthographic and environment are on it)");
+            return fail(PBRT_E_UNSUPPORTED, "camera kind outside pbrt_gpu_scene_create_camera (perspective, orthographic and environment; the realistic camera goes through pbrt_gpu_scene_create_lens)");
         if (camera->kind == PBRT_CAMERA_ENVIRONMENT && (camera->full_resolution[0] == 0 || camera->full_resolution[1] == 0))
             return fail(PBRT_E_INVALID, "environment camera with a zero full_resolution");
         P.cam_kind = camera->kind;
@@ -1558,13 +1610,14 @@ static int build_finish(const ScenePrep& P, std::vector<SceneBuild>& builds, uin
     sc->cam_mo = P.cam_mo;
     sc->cam_kind = P.cam_kind;
     sc->env_res = P.env_res;
+    sc->lens = P.lens;
     CK(cudaDeviceSynchronize());
     return PBRT_OK;
 }
 
 // The scene on devices[0..n) (distinct, already checked by the caller): out[k] is the replica on devices[k], or every out[k] is null.
-static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices, uint32_t n,
-                         PbrtScene** out) {
+static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const PbrtRealisticLens* lens,
+                         const int* devices, uint32_t n, PbrtScene** out) {
     static const int timing = getenv("PB_TIMING") ? atoi(getenv("PB_TIMING")) : 0;  // 1: every call; 2: only calls slower than 100 ms
     const auto t_enter = std::chrono::steady_clock::now();
     std::string timing_log;
@@ -1578,7 +1631,7 @@ static int create_scenes(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion
         if (mode == 2 && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() > 100.0) fputs(log.c_str(), stderr); } } slow_dump{timing_log, t_enter, timing};
     for (uint32_t k = 0; k < n; ++k) out[k] = nullptr;
     ScenePrep P;
-    int rc = scene_prepare(desc, motion, camera, P);
+    int rc = scene_prepare(desc, motion, camera, lens, P);
     if (rc != PBRT_OK) return rc;
     since("host preparation");
     for (uint32_t k = 0; k < n; ++k) {
@@ -1653,12 +1706,12 @@ extern "C" {
 
 int pbrt_gpu_scene_create(const PbrtSceneDesc* desc, int device, PbrtScene** out) {
     if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    return create_scenes(desc, nullptr, nullptr, &device, 1, out);
+    return create_scenes(desc, nullptr, nullptr, nullptr, &device, 1, out);
 }
 
 int pbrt_gpu_scene_create_motion(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, int device, PbrtScene** out) {
     if (!desc || !out) return fail(PBRT_E_INVALID, "null argument");
-    return create_scenes(desc, motion, nullptr, &device, 1, out);
+    return create_scenes(desc, motion, nullptr, nullptr, &device, 1, out);
 }
 
 int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const int* devices, uint32_t n_devices, PbrtScene** out) {
@@ -1667,13 +1720,18 @@ int pbrt_gpu_scene_create_multi(const PbrtSceneDesc* desc, const PbrtMotionDesc*
 
 int pbrt_gpu_scene_create_camera(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const int* devices,
                                  uint32_t n_devices, PbrtScene** out) {
+    return pbrt_gpu_scene_create_lens(desc, motion, camera, nullptr, devices, n_devices, out);
+}
+
+int pbrt_gpu_scene_create_lens(const PbrtSceneDesc* desc, const PbrtMotionDesc* motion, const PbrtCameraModel* camera, const PbrtRealisticLens* lens,
+                               const int* devices, uint32_t n_devices, PbrtScene** out) {
     if (!desc || !devices || !out || n_devices == 0) return fail(PBRT_E_INVALID, "null argument or no device");
     for (uint32_t k = 0; k < n_devices; ++k) out[k] = nullptr;
     if (n_devices > 16) return fail(PBRT_E_UNSUPPORTED, "more than 16 devices");
     for (uint32_t k = 0; k < n_devices; ++k)
         for (uint32_t j = 0; j < k; ++j)
             if (devices[j] == devices[k]) return fail(PBRT_E_INVALID, "a device is listed twice (one replica per device)");
-    return create_scenes(desc, motion, camera, devices, n_devices, out);
+    return create_scenes(desc, motion, camera, lens, devices, n_devices, out);
 }
 
 int pbrt_gpu_host_register(const void* ptr, uint64_t bytes) {
@@ -1888,6 +1946,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         for (int i = 0; i < 4; ++i) CK(X.f4[i].alloc(cap));
         CK(X.rays.alloc(2 * (cap + 2 * cap_nee)));
         CK(X.sobol.alloc(cap)); CK(X.dim.alloc(cap)); CK(X.pfilm.alloc(cap));
+        if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
         CK(X.queue[0].alloc(cap)); CK(X.counts.alloc(8 + PB_SHADE_CLASSES));
         DirectBufs& D = scr->direct;
         const bool dinst = sc->d.n_instances > 0;
@@ -1970,7 +2029,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
                 const auto raygen = raygen_kernel(sc);
                 raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, sc->nib.p, std::max(raygen_chunks, dd.n_chunks), sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count,
-                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo, sc->env_res);
+                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
                 launches++;
                 // the recursion's length is decided on the device (the active word = camera samples that still need an iteration).  The
                 // host reads that word poll_lag() iterations late (see there: 0 by default, measured): with a lag of 1 iteration i + 1 is
@@ -2007,7 +2066,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                     }
                     if (iter > 100000u) return fail(PBRT_E_CUDA, "direct integrator did not terminate");
                 }
-                k_resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples);
+                const auto resolve = resolve_kernel(sc);
+                resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples, X.cam_weight.p);
                 launches++;
             }
         CK(cudaGetLastError());
@@ -2043,6 +2103,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         CK(X.rays.alloc(2 * std::max(cap_paths, cap_rays)));
         CK(X.occl.alloc(cap_rays)); CK(X.ao_weight.alloc(cap_rays));
         CK(X.sobol.alloc(cap_paths)); CK(X.dim.alloc(cap_paths)); CK(X.pfilm.alloc(cap_paths));
+        if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap_paths));
         CK(X.queue[0].alloc(cap_paths)); CK(X.counts.alloc(8 + PB_SHADE_CLASSES));
         DPaths ps;
         std::memset(&ps, 0, sizeof ps);
@@ -2082,7 +2143,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
                 const auto raygen = raygen_kernel(sc);
                 raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count, X.rays.p, d_nrays,
-                                                        sc->counters.p, sc->cam_mo, sc->env_res);
+                                                        sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
                 launches++;
                 int rc = trace();
                 if (rc != PBRT_OK) return rc;
@@ -2098,7 +2159,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 launches++;
                 if ((rc = trace()) != PBRT_OK) return rc;
                 k_ao_resolve<<<(n + 255) / 256, 256, 0, st>>>(ps, bi, ao_n, X.ao_weight.p, X.occl.p);
-                k_resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples);
+                const auto resolve = resolve_kernel(sc);
+                resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples, X.cam_weight.p);
                 launches += 2;
             }
         CK(cudaGetLastError());
@@ -2308,6 +2370,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             }
             CK(X.rays.alloc(2 * 3 * cap));  // up to three rays (path, MIS, shadow) per slot and bounce
             CK(X.pfilm.alloc(cap));
+            if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
             CK(X.queue[0].alloc(cap)); CK(X.queue[1].alloc(cap)); CK(X.counts.alloc(8 + 2 * PB_SHADE_CLASSES));
             CK(X.cls_queue.alloc((size_t)PB_SHADE_CLASSES * cap));
             CK(X.g_state.alloc(nvox)); CK(X.g_func.alloc(grid_rows * std::max<size_t>(nl, 1))); CK(X.g_cdf.alloc(grid_rows * (nl + 1)));
@@ -2483,13 +2546,14 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             if (spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
             const auto raygen = raygen_kernel(sc);
             raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays,
-                                                      sc->counters.p, sc->cam_mo, sc->env_res);
+                                                      sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
             launches++;
             return PBRT_OK;
         };
         auto enqueue_end = [&](int c, const BatchInfo& bi) -> int {
             Live& V = live[c];
-            k_resolve<<<(bi.n_pixels + 255) / 256, 256, 0, V.s>>>(rp, V.ps, bi, scr->filter_table.p, d_film, d_samples);
+            const auto resolve = resolve_kernel(sc);
+            resolve<<<(bi.n_pixels + 255) / 256, 256, 0, V.s>>>(rp, V.ps, bi, scr->filter_table.p, d_film, d_samples, scr->ctx[c].cam_weight.p);
             launches++;
             return PBRT_OK;
         };
@@ -2915,6 +2979,38 @@ int pbrt_gpu_kat_animated_interpolate(int device, const PbrtAnimatedTransform* a
     g_launches++;
     CK(cudaMemcpy(m_out, dm.p, (size_t)n * 64, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(m_inv_out, dmi.p, (size_t)n * 64, cudaMemcpyDeviceToHost));
+    return PBRT_OK;
+}
+
+// Known-answer hook: the realistic camera's generate_ray_differential on the device (pb_lens.cuh), for a scene from
+// pbrt_gpu_scene_create_lens.  Not part of the render path.
+int pbrt_gpu_kat_realistic_rays(PbrtScene* sc, uint32_t n, const float* p_film, const float* p_lens, const float* time, float* o, float* d,
+                                float* weight, float* rx_o, float* ry_o, float* rx_d, float* ry_d) {
+    if (!sc || (n && (!p_film || !p_lens || !time || !o || !d || !weight || !rx_o || !ry_o || !rx_d || !ry_d))) return fail(PBRT_E_INVALID, "null argument");
+    if (sc->cam_kind != PBRT_CAMERA_REALISTIC) return fail(PBRT_E_INVALID, "scene without a realistic camera");
+    if (n == 0) return PBRT_OK;
+    CK(cudaSetDevice(sc->device));
+    std::vector<float4> in(n);
+    for (uint32_t i = 0; i < n; ++i) in[i] = make_float4(p_film[2 * i], p_film[2 * i + 1], p_lens[2 * i], p_lens[2 * i + 1]);
+    DevBuf<float4> din;
+    DevBuf<float> dt, dout;
+    CK(din.alloc(n)); CK(dt.alloc(n)); CK(dout.alloc(19 * (size_t)n));
+    CK(cudaMemcpy(din.p, in.data(), (size_t)n * 16, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dt.p, time, (size_t)n * 4, cudaMemcpyHostToDevice));
+    k_kat_realistic<<<(n + 255) / 256, 256>>>(sc->d, sc->lens, sc->cam_mo, sc->cam_motion ? 1u : 0u, din.p, dt.p, n, dout.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    g_launches++;
+    std::vector<float> h(19 * (size_t)n);
+    CK(cudaMemcpy(h.data(), dout.p, h.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < n; ++i) {
+        const float* r = h.data() + 19 * (size_t)i;
+        for (int k = 0; k < 3; ++k) {
+            o[3 * i + k] = r[k]; d[3 * i + k] = r[3 + k];
+            rx_o[3 * i + k] = r[7 + k]; ry_o[3 * i + k] = r[10 + k]; rx_d[3 * i + k] = r[13 + k]; ry_d[3 * i + k] = r[16 + k];
+        }
+        weight[i] = r[6];
+    }
     return PBRT_OK;
 }
 

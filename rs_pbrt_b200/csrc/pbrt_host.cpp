@@ -10,6 +10,8 @@
 #include <limits>
 #include <memory>
 #include <string>
+#include <system_error>
+#include <thread>
 #include <vector>
 
 #include "../../include/pbrt_host.h"
@@ -316,6 +318,10 @@ struct PbrtHost {
     bool have_camera = false;
     PbrtCamera cam;
     PbrtCameraModel cam_model = {PBRT_CAMERA_PERSPECTIVE, {0, 0}};
+    float film_diagonal = 0.035f;                 // Film.diagonal in metres (film.rs:250: "diagonal" 35 mm)
+    std::vector<PbrtLensElement> lens_elements;   // the realistic camera, as RealisticCamera::new leaves it
+    std::vector<float> pupil_bounds;
+    PbrtRealisticLens lens = {};
     int pixel_samples = 16;
     uint32_t sampler = PBRT_SAMPLER_SOBOL;
     bool sample_at_pixel_center = false;
@@ -788,6 +794,226 @@ int pbrt_host_camera_environment(PbrtHost* h, float shutter_open, float shutter_
     return 0;
 }
 
+// ---- RealisticCamera::new (src/cameras/realistic.rs:50-144) ---------------------------------------------------------------------
+namespace lens {
+struct R { float o[3], d[3]; };
+// Transform::scale(1, 1, -1).transform_ray, with the origin error offset (transform.rs:538-549, 662-692)
+void flip(R& r) {
+    const float x = r.o[0], y = r.o[1], z = r.o[2];
+    float o[3] = {1.0f * x + 0.0f * y + 0.0f * z + 0.0f, 0.0f * x + 1.0f * y + 0.0f * z + 0.0f, 0.0f * x + 0.0f * y + -1.0f * z + 0.0f};
+    const float w = 0.0f * x + 0.0f * y + 0.0f * z + 1.0f;
+    const float g3 = (3.0f * (std::numeric_limits<float>::epsilon() * 0.5f)) / (1.0f - 3.0f * (std::numeric_limits<float>::epsilon() * 0.5f));
+    const float e[3] = {(std::fabs(1.0f * x) + std::fabs(0.0f * y) + std::fabs(0.0f * z) + std::fabs(0.0f)) * g3,
+                        (std::fabs(0.0f * x) + std::fabs(1.0f * y) + std::fabs(0.0f * z) + std::fabs(0.0f)) * g3,
+                        (std::fabs(0.0f * x) + std::fabs(0.0f * y) + std::fabs(-1.0f * z) + std::fabs(0.0f)) * g3};
+    if (w != 1.0f) { const float inv = 1.0f / w; for (float& v : o) v *= inv; }
+    const float d[3] = {1.0f * r.d[0] + 0.0f * r.d[1] + 0.0f * r.d[2], 0.0f * r.d[0] + 1.0f * r.d[1] + 0.0f * r.d[2],
+                        0.0f * r.d[0] + 0.0f * r.d[1] + -1.0f * r.d[2]};
+    const float ls = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+    if (ls > 0.0f) {
+        const float dt = (std::fabs(d[0]) * e[0] + std::fabs(d[1]) * e[1] + std::fabs(d[2]) * e[2]) / ls;
+        for (int k = 0; k < 3; ++k) o[k] += d[k] * dt;
+    }
+    for (int k = 0; k < 3; ++k) { r.o[k] = o[k]; r.d[k] = d[k]; }
+}
+// intersect_spherical_element (:328-365) with quadratic's f64 discriminant (pbrt.rs:248-268)
+bool sphere(float radius, float z_center, const R& r, float& t, float n[3]) {
+    const float oc[3] = {r.o[0] - 0.0f, r.o[1] - 0.0f, r.o[2] - z_center};
+    const float a = r.d[0] * r.d[0] + r.d[1] * r.d[1] + r.d[2] * r.d[2];
+    const float b = 2.0f * (r.d[0] * oc[0] + r.d[1] * oc[1] + r.d[2] * oc[2]);
+    const float c = oc[0] * oc[0] + oc[1] * oc[1] + oc[2] * oc[2] - radius * radius;
+    const double disc = (double)b * (double)b - 4.0 * (double)a * (double)c;
+    if (disc < 0.0) return false;
+    const double rd = std::sqrt(disc);
+    const double q = b < 0.0f ? -0.5 * ((double)b - rd) : -0.5 * ((double)b + rd);
+    float t0 = (float)q / a, t1 = c / (float)q;
+    if (t0 > t1) std::swap(t0, t1);
+    t = ((r.d[2] > 0.0f) ^ (radius < 0.0f)) ? std::fmin(t0, t1) : std::fmax(t0, t1);
+    if (t < 0.0f) return false;
+    float v[3] = {oc[0] + r.d[0] * t, oc[1] + r.d[1] * t, oc[2] + r.d[2] * t};
+    const float inv = 1.0f / std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    for (int k = 0; k < 3; ++k) v[k] *= inv;
+    const bool flip_n = v[0] * -r.d[0] + v[1] * -r.d[1] + v[2] * -r.d[2] < 0.0f;
+    for (int k = 0; k < 3; ++k) n[k] = flip_n ? -v[k] : v[k];
+    return true;
+}
+// refract (reflection.rs:1897-1910) of -d, normalised, through n
+bool refract(const R& r, const float n[3], float eta, float wt[3]) {
+    const float l = std::sqrt(r.d[0] * r.d[0] + r.d[1] * r.d[1] + r.d[2] * r.d[2]), inv = 1.0f / l;
+    const float wi[3] = {-r.d[0] * inv, -r.d[1] * inv, -r.d[2] * inv};
+    const float cos_i = n[0] * wi[0] + n[1] * wi[1] + n[2] * wi[2];
+    const float sin2_t = eta * eta * std::fmax(0.0f, 1.0f - cos_i * cos_i);
+    if (sin2_t >= 1.0f) return false;
+    const float cos_t = std::sqrt(1.0f - sin2_t);
+    for (int k = 0; k < 3; ++k) wt[k] = -wi[k] * eta + n[k] * (eta * cos_i - cos_t);
+    return true;
+}
+// trace_lenses_from_film (:266-327) / trace_lenses_from_scene (:366-421); r: camera space in, camera space out
+bool trace(const std::vector<PbrtLensElement>& el, R& r, bool from_film) {
+    flip(r);
+    const size_t ne = el.size();
+    float element_z = 0.0f;
+    if (!from_film) for (const auto& e : el) element_z += e.thickness;
+    if (!from_film) element_z = -element_z;
+    for (size_t k = 0; k < ne; ++k) {
+        const size_t i = from_film ? ne - 1 - k : k;
+        const PbrtLensElement& e = el[i];
+        if (from_film) element_z -= e.thickness;
+        float t = 0.0f, n[3] = {0.0f, 0.0f, 0.0f};
+        const bool is_stop = e.curvature_radius == 0.0f;
+        if (is_stop) {
+            if (from_film && r.d[2] >= 0.0f) return false;
+            t = (element_z - r.o[2]) / r.d[2];
+        } else if (!sphere(e.curvature_radius, element_z + e.curvature_radius, r, t, n)) return false;
+        if (!(t >= 0.0f)) return false;  // the reference asserts
+        const float p[3] = {r.o[0] + r.d[0] * t, r.o[1] + r.d[1] * t, r.o[2] + r.d[2] * t};
+        if (p[0] * p[0] + p[1] * p[1] > e.aperture_radius * e.aperture_radius) return false;
+        for (int q = 0; q < 3; ++q) r.o[q] = p[q];
+        if (!is_stop) {
+            float eta;
+            if (from_film) eta = e.eta / ((i > 0 && el[i - 1].eta != 0.0f) ? el[i - 1].eta : 1.0f);
+            else eta = ((i == 0 || el[i - 1].eta == 0.0f) ? 1.0f : el[i - 1].eta) / (e.eta != 0.0f ? e.eta : 1.0f);
+            float w[3];
+            if (!refract(r, n, eta, w)) return false;
+            for (int q = 0; q < 3; ++q) r.d[q] = w[q];
+        }
+        if (!from_film) element_z += e.thickness;
+    }
+    flip(r);
+    return true;
+}
+float radical_inverse2(uint64_t a) {  // lowdiscrepancy.rs:1126-1134: reverse_bits_64(a) as f32 * 2^-64
+    uint64_t v = 0;
+    for (int b = 0; b < 64; ++b) v |= ((a >> b) & 1u) << (63 - b);
+    return (float)v * 0x1.0p-64f;
+}
+float radical_inverse3(uint64_t a) {  // lowdiscrepancy.rs:1082-1096
+    const float inv_base = 1.0f / 3.0f;
+    uint64_t reversed = 0;
+    float inv_base_n = 1.0f;
+    while (a != 0) {
+        const uint64_t next = a / 3, digit = a - next * 3;
+        reversed = reversed * 3 + digit;
+        inv_base_n *= inv_base;
+        a = next;
+    }
+    return std::fmin((float)reversed * inv_base_n, 0x1.fffffep-1f);
+}
+float lerp(float t, float a, float b) { return a * (1.0f - t) + b * t; }
+// bound_exit_pupil (:573-652).  The running box starts as Bounds2f::default(), the zero box (geometry.rs:1865), so every bin's
+// bounds contain the optical axis.  A point inside the running box never changes it, so the visiting order does not matter.
+void bound_exit_pupil(const std::vector<PbrtLensElement>& el, float x0, float x1, float out[4]) {
+    const int n_samples = 1024 * 1024;
+    float b[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    int n_exiting = 0;
+    const float rr = el.back().aperture_radius, rear_z = el.back().thickness;
+    const float pr[4] = {-1.5f * rr, -1.5f * rr, 1.5f * rr, 1.5f * rr};
+    for (int i = 0; i < n_samples; ++i) {
+        const float fx = lerp(((float)i + 0.5f) / (float)n_samples, x0, x1);
+        const float rx = lerp(radical_inverse2((uint64_t)i), pr[0], pr[2]), ry = lerp(radical_inverse3((uint64_t)i), pr[1], pr[3]);
+        bool pass = rx >= b[0] && rx <= b[2] && ry >= b[1] && ry <= b[3];
+        if (!pass) {
+            R r = {{fx, 0.0f, 0.0f}, {rx - fx, ry - 0.0f, rear_z - 0.0f}};
+            pass = trace(el, r, true);
+        }
+        if (pass) {
+            b[0] = std::fmin(b[0], rx); b[1] = std::fmin(b[1], ry); b[2] = std::fmax(b[2], rx); b[3] = std::fmax(b[3], ry);
+            ++n_exiting;
+        }
+    }
+    if (n_exiting == 0) { std::memcpy(out, pr, 16); return; }
+    const float dx = pr[2] - pr[0], dy = pr[3] - pr[1];
+    const float delta = 2.0f * std::sqrt(dx * dx + dy * dy) / std::sqrt((float)n_samples);
+    out[0] = b[0] - delta; out[1] = b[1] - delta; out[2] = b[2] + delta; out[3] = b[3] + delta;
+}
+// The 64 bins of RealisticCamera::new (:100-139) on host threads; false (and g_herr set) when a thread cannot be started.
+bool exit_pupil_bounds(const std::vector<PbrtLensElement>& el, float diag, float* bounds) {
+    const unsigned nt = std::max(1u, std::min(64u, std::thread::hardware_concurrency()));
+    std::vector<std::thread> pool;
+    auto work = [&](unsigned t, unsigned stride) {
+        for (unsigned i = t; i < 64; i += stride) {
+            const float r0 = (float)i / 64.0f * diag / 2.0f, r1 = (float)(i + 1) / 64.0f * diag / 2.0f;
+            bound_exit_pupil(el, r0, r1, bounds + 4 * i);
+        }
+    };
+    try {
+        for (unsigned t = 0; t < nt; ++t) pool.emplace_back(work, t, nt);
+    } catch (const std::system_error& e) {
+        for (auto& th : pool) th.join();
+        g_herr = std::string("cannot start a thread for the exit pupil bounds: ") + e.what();
+        return false;
+    }
+    for (auto& th : pool) th.join();
+    return true;
+}
+}  // namespace lens
+
+int pbrt_host_lens_exit_pupil(const PbrtLensElement* elements, int n_elements, float film_diagonal_m, float* bounds) {
+    if (!elements || !bounds || n_elements <= 0) return hfail(PBRT_E_INVALID, "null argument or no lens element");
+    if (!std::isfinite(film_diagonal_m) || !(film_diagonal_m > 0.0f)) return hfail(PBRT_E_INVALID, "film diagonal must be > 0");
+    const std::vector<PbrtLensElement> el(elements, elements + n_elements);
+    return lens::exit_pupil_bounds(el, film_diagonal_m, bounds) ? 0 : PBRT_E_INVALID;
+}
+
+int pbrt_host_film_diagonal(PbrtHost* h, float mm) {  // Film "diagonal" (film.rs:250, millimetres; Film::new keeps metres)
+    if (!h) return hfail(PBRT_E_INVALID, "null argument");
+    if (!std::isfinite(mm) || !(mm > 0.0f)) return hfail(PBRT_E_INVALID, "film diagonal must be > 0");
+    h->film_diagonal = mm * 0.001f;
+    return 0;
+}
+
+int pbrt_host_camera_realistic(PbrtHost* h, const float* lens_mm, int n_values, float aperture_diameter, float focus_distance, int simple_weighting,
+                               float shutter_open, float shutter_close) {
+    if (!h || (n_values && !lens_mm)) return hfail(PBRT_E_INVALID, "null argument");
+    if (n_values <= 0 || n_values % 4 != 0) return hfail(PBRT_E_INVALID, "the lens file must hold a positive multiple of four values");
+    if (!(shutter_close >= shutter_open)) return hfail(PBRT_E_INVALID, "shutterclose < shutteropen");
+    std::vector<PbrtLensElement> el;
+    for (int i = 0; i < n_values; i += 4) {  // :62-80: mm -> m; the stop takes "aperturediameter" unless that is larger
+        float diameter = lens_mm[i + 3];
+        if (lens_mm[i] == 0.0f && !(aperture_diameter > lens_mm[i + 3])) diameter = aperture_diameter;
+        el.push_back(PbrtLensElement{lens_mm[i] * 0.001f, lens_mm[i + 1] * 0.001f, lens_mm[i + 2], diameter * 0.001f / 2.0f});
+    }
+    if (el.size() > PBRT_MAX_LENS_ELEMENTS) return hfail(PBRT_E_UNSUPPORTED, "more lens elements than PBRT_MAX_LENS_ELEMENTS");
+    // focus_thick_lens (:483-499) with compute_thick_lens_approximation (:444-482).  focus_binary_search (:500-521) also runs in
+    // the reference, but its result is discarded (`_fb`) and it changes nothing, so it is not restated.
+    const float x = 0.001f * h->film_diagonal;
+    float front_z = 0.0f;
+    for (const auto& e : el) front_z += e.thickness;
+    float pz[2], fz[2];
+    lens::R r_scene = {{x, 0.0f, front_z + 1.0f}, {0.0f, 0.0f, -1.0f}}, r_film = r_scene;
+    if (!lens::trace(el, r_film, false)) return hfail(PBRT_E_INVALID, "no ray from the scene reaches the film for the thick lens approximation");
+    auto cardinal = [&](const lens::R& in, const lens::R& out, int idx) {  // compute_cardinal_points (:431-443)
+        const float tf = -out.o[0] / out.d[0];
+        fz[idx] = -(out.o[2] + out.d[2] * tf);
+        const float tp = (in.o[0] - out.o[0]) / out.d[0];
+        pz[idx] = -(out.o[2] + out.d[2] * tp);
+    };
+    cardinal(r_scene, r_film, 0);
+    lens::R r_film2 = {{x, 0.0f, el.back().thickness - 1.0f}, {0.0f, 0.0f, 1.0f}}, r_scene2 = r_film2;
+    if (!lens::trace(el, r_scene2, true)) return hfail(PBRT_E_INVALID, "no ray from the film reaches the scene for the thick lens approximation");
+    cardinal(r_film2, r_scene2, 1);
+    const float f = fz[0] - pz[0], z = -focus_distance;
+    const float c = (pz[1] - z - pz[0]) * (pz[1] - z - 4.0f * f - pz[0]);
+    if (!(c > 0.0f)) return hfail(PBRT_E_INVALID, "focus distance too short for this lens");
+    const float delta = 0.5f * (pz[1] - z + pz[0] - std::sqrt(c));
+    el.back().thickness = el.back().thickness + delta;
+    // exit_pupil_bounds (:100-139), 64 bins on host threads
+    std::vector<float> bounds(4 * 64);
+    const float diag = h->film_diagonal;
+    if (!lens::exit_pupil_bounds(el, diag, bounds.data())) return PBRT_E_INVALID;
+    h->lens_elements = el;
+    h->pupil_bounds = bounds;
+    h->lens = PbrtRealisticLens{h->lens_elements.data(), (uint32_t)el.size(), h->pupil_bounds.data(), diag, simple_weighting ? 1u : 0u};
+    const M4 ident = m4_identity();  // RealisticCamera reads neither raster_to_camera nor the thin lens
+    std::memcpy(h->cam.raster_to_camera, ident.m, 64);
+    std::memcpy(h->cam.camera_to_world, h->camera_to_world.m, 64);
+    h->cam.lens_radius = 0.0f; h->cam.focal_distance = 1e30f;
+    h->cam.shutter_open = shutter_open; h->cam.shutter_close = shutter_close;
+    h->cam_model = PbrtCameraModel{PBRT_CAMERA_REALISTIC, {(uint32_t)h->xres, (uint32_t)h->yres}};
+    h->have_camera = true;
+    return 0;
+}
+
 int pbrt_host_sampler_sobol(PbrtHost* h, int pixel_samples) {  // sobol.rs:37-45: rounded up to a power of two
     if (!h || pixel_samples <= 0) return hfail(PBRT_E_INVALID, "bad pixel sample count");
     int v = 1;
@@ -1042,11 +1268,14 @@ const PbrtSceneDesc* pbrt_host_scene_desc(const PbrtHost* h) { return (h && h->b
 const PbrtMotionDesc* pbrt_host_motion_desc(const PbrtHost* h) { return (h && h->built && h->motion.camera) ? &h->motion : nullptr; }
 const PbrtRenderParams* pbrt_host_render_params(const PbrtHost* h) { return (h && h->built) ? &h->rp : nullptr; }
 const PbrtCameraModel* pbrt_host_camera_model(const PbrtHost* h) { return (h && h->built) ? &h->cam_model : nullptr; }
+const PbrtRealisticLens* pbrt_host_lens(const PbrtHost* h) {
+    return (h && h->built && h->cam_model.kind == PBRT_CAMERA_REALISTIC) ? &h->lens : nullptr;
+}
 
 int pbrt_host_render(PbrtHost* h, int device, const int32_t* pixel_rect, PbrtStats* stats) {
     if (!h || !h->built) return hfail(PBRT_E_INVALID, "pbrt_host_world_end has not run");
     PbrtScene* sc = nullptr;
-    int rc = pbrt_gpu_scene_create_camera(&h->desc, pbrt_host_motion_desc(h), pbrt_host_camera_model(h), &device, 1, &sc);
+    int rc = pbrt_gpu_scene_create_lens(&h->desc, pbrt_host_motion_desc(h), pbrt_host_camera_model(h), pbrt_host_lens(h), &device, 1, &sc);
     if (rc != PBRT_OK) return hfail(rc, pbrt_gpu_last_error());
     const int32_t* rect = pixel_rect ? pixel_rect : h->rp.sample_bounds;
     rc = pbrt_gpu_render(sc, &h->rp, rect, h->film.data(), stats);

@@ -241,6 +241,20 @@ class HostScene:
         self.log.append(("camera_environment", dict(shutteropen=float(shutteropen), shutterclose=float(shutterclose))))
         self._ck(self.L.pbrt_host_camera_environment(self.h, shutteropen, shutterclose))
 
+    def film_diagonal(self, mm=35.0):
+        """Film "diagonal" in millimetres (the realistic camera's film size); call after film() and before the camera."""
+        self.log.append(("film_diagonal", dict(mm=float(mm))))
+        self._ck(self.L.pbrt_host_film_diagonal(self.h, mm))
+
+    def camera_realistic(self, lens, aperturediameter=1.0, focusdistance=10.0, simpleweighting=True, shutteropen=0.0, shutterclose=1.0):
+        """Camera "realistic" (the reference's defaults): `lens` is the lens file's numbers, rows {radius, thickness, eta, diameter} in
+        mm; call after film() (and film_diagonal())."""
+        v = np.ascontiguousarray(np.asarray(lens, np.float32).ravel())
+        self.log.append(("camera_realistic", dict(lens=v.copy(), aperturediameter=float(aperturediameter), focusdistance=float(focusdistance),
+                                                  simpleweighting=bool(simpleweighting), shutteropen=float(shutteropen), shutterclose=float(shutterclose))))
+        self._ck(self.L.pbrt_host_camera_realistic(self.h, _fptr(v), int(v.size), aperturediameter, focusdistance, 1 if simpleweighting else 0,
+                                                   shutteropen, shutterclose))
+
     def sampler(self, pixelsamples=16, name="sobol", samplepixelcenter=False):
         """Sampler "sobol" (pixelsamples rounded up to a power of two) or "halton"."""
         self.log.append(("sampler", dict(pixelsamples=int(pixelsamples), name=name, samplepixelcenter=bool(samplepixelcenter))))
@@ -325,6 +339,12 @@ class HostScene:
         p = self.L.pbrt_host_camera_model(self.h)
         return p if p else None
 
+    @property
+    def lens(self):
+        """The PbrtRealisticLens of the built scene (a realistic camera), for GpuScene(lens=...) and create_multi; None otherwise."""
+        p = self.L.pbrt_host_lens(self.h)
+        return p if p else None
+
     def film_shape(self):
         cb = self.params.contents.cropped_pixel_bounds
         return (cb[3] - cb[1], cb[2] - cb[0])
@@ -361,12 +381,16 @@ class HostScene:
 class GpuScene:
     """A scene resident on one GPU: pbrt_gpu_scene_create / render / intersect (include/pbrt_gpu.h).  `motion`: a PbrtMotionDesc (or a
     pointer to one, e.g. HostScene.motion) for pbrt_gpu_scene_create_motion.  `camera`: a PbrtCameraModel (or a pointer to one, e.g.
-    HostScene.camera_model) for pbrt_gpu_scene_create_camera; None is the perspective camera."""
+    HostScene.camera_model) for pbrt_gpu_scene_create_camera; None is the perspective camera.  `lens`: a PbrtRealisticLens (or a
+    pointer to one, e.g. HostScene.lens) with a realistic camera model, for pbrt_gpu_scene_create_lens."""
 
-    def __init__(self, desc, device=0, lib=None, motion=None, camera=None):
+    def __init__(self, desc, device=0, lib=None, motion=None, camera=None, lens=None):
         self.L = lib if lib is not None else _abi.load()  # `lib`: tests may pass another build of the same C ABI
         self.handle = C.c_void_p()
-        if camera is not None:
+        if lens is not None:
+            dev = C.c_int(device)
+            rc = self.L.pbrt_gpu_scene_create_lens(desc, _ptr(motion), _ptr(camera), _ptr(lens), C.byref(dev), 1, C.byref(self.handle))
+        elif camera is not None:
             dev = C.c_int(device)
             rc = self.L.pbrt_gpu_scene_create_camera(desc, _ptr(motion), _ptr(camera), C.byref(dev), 1, C.byref(self.handle))
         elif motion is not None:
@@ -420,6 +444,20 @@ class GpuScene:
         st = _abi.PbrtStats()
         self._ck(self.L.pbrt_gpu_render_tiles_device(self.handle, params, int(part), int(n_parts), C.c_void_p(d_film_ptr), C.c_void_p(stream or 0), C.byref(st)))
         return st.as_dict()
+
+    def kat_realistic_rays(self, p_film, p_lens, time):
+        """pbrt_gpu_kat_realistic_rays: the device's generate_ray_differential of a realistic-camera scene for each camera sample ->
+        dict of float32 arrays o, d, rx_o, ry_o, rx_d, ry_d (n, 3) and weight (n,)."""
+        pf = np.ascontiguousarray(p_film, np.float32).reshape(-1, 2)
+        n = pf.shape[0]
+        pl = np.ascontiguousarray(p_lens, np.float32).reshape(n, 2)
+        t = np.ascontiguousarray(time, np.float32).reshape(n)
+        out = {k: np.zeros((n, 3), np.float32) for k in ("o", "d", "rx_o", "ry_o", "rx_d", "ry_d")}
+        out["weight"] = np.zeros(n, np.float32)
+        rc = self.L.pbrt_gpu_kat_realistic_rays(self.handle, n, _fptr(pf), _fptr(pl), _fptr(t), *[_fptr(out[k]) for k in ("o", "d", "weight", "rx_o", "ry_o", "rx_d", "ry_d")])
+        if rc != 0:
+            raise PbrtError(rc, self.L.pbrt_gpu_last_error().decode())
+        return out
 
     def render_samples(self, params, rect):
         r = self._rect(params, rect)
@@ -482,15 +520,17 @@ def _ptr(x):
     return x if x is None or isinstance(x, C._Pointer) else C.pointer(x)
 
 
-def create_multi(desc, devices, motion=None, lib=None, camera=None):
+def create_multi(desc, devices, motion=None, lib=None, camera=None, lens=None):
     """pbrt_gpu_scene_create_multi: the scene on every device of `devices` in one call, each large array crossing PCIe once; returns one
-    GpuScene per device, in the order given.  `motion`, `camera`: as for GpuScene (a camera model goes through
-    pbrt_gpu_scene_create_camera)."""
+    GpuScene per device, in the order given.  `motion`, `camera`, `lens`: as for GpuScene (a camera model goes through
+    pbrt_gpu_scene_create_camera, a lens through pbrt_gpu_scene_create_lens)."""
     L = lib if lib is not None else _abi.load()
     devs = (C.c_int * len(devices))(*[int(d) for d in devices])
     handles = (C.c_void_p * max(len(devices), 1))()
     motion = _ptr(motion)
-    if camera is not None:
+    if lens is not None:
+        rc = L.pbrt_gpu_scene_create_lens(desc, motion, _ptr(camera), _ptr(lens), devs, len(devices), handles)
+    elif camera is not None:
         rc = L.pbrt_gpu_scene_create_camera(desc, motion, _ptr(camera), devs, len(devices), handles)
     else:
         rc = L.pbrt_gpu_scene_create_multi(desc, motion, devs, len(devices), handles)

@@ -167,7 +167,7 @@ def write(h, path, ply_threshold=2000):
     mesh_i = 0
     in_object = False
     objects = 0
-    film = sampler = integrator = camera = look = camera_end = times = None
+    film = sampler = integrator = camera = look = camera_end = times = diagonal = None
     for name, a in h.log:
         if name == "material":
             materials.append(a)
@@ -275,8 +275,10 @@ def write(h, path, ply_threshold=2000):
             camera_end = a["m"]
         elif name == "film":
             film = a
-        elif name in ("camera", "camera_orthographic", "camera_environment"):
+        elif name in ("camera", "camera_orthographic", "camera_environment", "camera_realistic"):
             camera = dict(a, kind=name)
+        elif name == "film_diagonal":
+            diagonal = a["mm"]
         elif name == "sampler":
             sampler = a
         elif name == "integrator":
@@ -297,6 +299,12 @@ def write(h, path, ply_threshold=2000):
         s = 'Camera "orthographic"'
     elif kind == "camera_environment":
         s = 'Camera "environment"'
+    elif kind == "camera_realistic":  # the lens file in read_float_file's format (floatfile.rs): rows {radius, thickness, eta, diameter} in mm
+        fn = "%s_lens.dat" % stem
+        rows = np.asarray(c["lens"], np.float32).reshape(-1, 4)
+        (path.parent / fn).write_text("# radius thickness eta diameter (mm)\n" + "".join("%s\n" % _nums(r) for r in rows))
+        s = 'Camera "realistic" "string lensfile" ["%s"] "float aperturediameter" [%r] "float focusdistance" [%r] "bool simpleweighting" ["%s"]' % (
+            fn, c["aperturediameter"], c["focusdistance"], "true" if c["simpleweighting"] else "false")
     else:
         s = 'Camera "perspective" "float fov" [%r]' % c.get("fov", 90.0)
     if (c.get("shutteropen", 0.0), c.get("shutterclose", 1.0)) != (0.0, 1.0):
@@ -325,6 +333,8 @@ def write(h, path, ply_threshold=2000):
     s = 'Film "image" "integer xresolution" [%d] "integer yresolution" [%d] "string filename" ["%s.png"]' % (f["xres"], f["yres"], stem)
     if f.get("crop") is not None:
         s += ' "float cropwindow" [%s]' % _nums(f["crop"])
+    if diagonal is not None:
+        s += ' "float diagonal" [%r]' % diagonal
     if np.isfinite(f.get("max_sample_luminance", float("inf"))):
         s += ' "float maxsampleluminance" [%r]' % f["max_sample_luminance"]
     pre.append(s)

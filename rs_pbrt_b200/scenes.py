@@ -79,10 +79,18 @@ def projector_transform(pos, target, up=(0.0, 1.0, 0.0)):
     return m
 
 
+# A 50 mm f/2 double-Gauss lens as a RealisticCamera lens file: rows {radius, thickness, eta, diameter} in mm, scene side first
+# (US patent 2,673,491, as tabulated in W. J. Smith, Modern Lens Design, p. 312, scaled from 100 mm to 50 mm).
+DGAUSS_50MM = [
+    [29.475, 3.76, 1.67, 25.2], [84.83, 0.12, 1.0, 25.2], [19.275, 4.025, 1.67, 23.0], [40.77, 3.275, 1.699, 23.0], [12.75, 5.705, 1.0, 18.0],
+    [0.0, 4.5, 0.0, 17.1], [-14.495, 1.18, 1.603, 17.0], [40.77, 6.065, 1.658, 20.0], [-20.385, 0.19, 1.0, 20.0], [437.065, 3.22, 1.717, 20.0],
+    [-39.73, 5.0, 1.0, 20.0]]
+
+
 def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filter="box", xwidth=0.5, ywidth=0.5, lensradius=0.0,
                 focaldistance=1e6, n_threads=8, crop=None, materials="matte", lights="area", sampler="sobol", samplepixelcenter=False, integrator="path", textures=None, lightsamples=1,
                 alpha=None, quantize_textures=False, camera_end=None, shutter=(0.0, 1.0), transform_times=(0.0, 1.0), camera="perspective",
-                screenwindow=None):
+                screenwindow=None, lensfile=None, aperturediameter=8.0, focusdistance=1000.0, simpleweighting=True, filmdiagonal=35.0):
     """Canonical Cornell box: 5 walls, short and tall block, ceiling light quad (2 triangles => 2 area lights, so
     the spatial light distribution is active).  32 triangles.  `materials="mixed"` swaps the blocks to glass /
     metal and the floor to plastic for BxDF coverage ("translucent", "mix": TranslucentMaterial / MixMaterial on blocks, floor and back wall).  `lights`: "area" (the ceiling quad only), "delta" (plus a point, a spot
@@ -97,7 +105,9 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
     and a card with `"float alpha" 0` (never hit by anything).  `quantize_textures`: every image texel is rounded to a multiple of 1/255, so
     that the scene equals its own .pbrt export (rs_pbrt reads images as 8-bit RGB; rs_pbrt_b200/pbrt_export.py).  `camera`:
     "perspective", "orthographic" (a view of the box's front, 560 units high, unless `screenwindow` says otherwise; lensradius /
-    focaldistance apply) or "environment" (a lat-long view of everything around a point inside the box, near its open front)."""
+    focaldistance apply), "environment" (a lat-long view of everything around a point inside the box, near its open front) or
+    "realistic" (the lens file `lensfile`, DGAUSS_50MM by default, with aperturediameter / focusdistance / simpleweighting and a film
+    of `filmdiagonal` mm)."""
     h = HostScene()
     if quantize_textures:
         _ti = h.texture_image
@@ -237,6 +247,10 @@ def cornell_box(xres=400, yres=400, spp=64, maxdepth=5, strategy="spatial", filt
                               screenwindow=screenwindow if screenwindow is not None else _screen_window(xres, yres, 280.0))
     elif camera == "environment":
         h.camera_environment(shutteropen=shutter[0], shutterclose=shutter[1])
+    elif camera == "realistic":
+        h.film_diagonal(filmdiagonal)
+        h.camera_realistic(DGAUSS_50MM if lensfile is None else lensfile, aperturediameter=aperturediameter, focusdistance=focusdistance,
+                           simpleweighting=simpleweighting, shutteropen=shutter[0], shutterclose=shutter[1])
     elif camera == "perspective":
         h.camera(fov=39.3077, lensradius=lensradius, focaldistance=focaldistance, shutteropen=shutter[0], shutterclose=shutter[1], screenwindow=screenwindow)
     else:
@@ -439,13 +453,14 @@ def _fbm(u, v, rng, octaves=6):
 
 
 def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, with_normals=True, n_threads=8, crop=None, integrator="path",
-           dolly=0.0, extra_light=None, camera="perspective"):
+           dolly=0.0, extra_light=None, camera="perspective", aperturediameter=6.0):
     """Ganesha stand-in (config C3): an fBm-displaced, vertically stretched UV sphere of 2*n_side^2 triangles
     (n_side=1468 -> 4.31 M) with per-vertex normals, on a ground quad, lit by 3 rectangular area lights
     (6 light triangles); matte statue + plastic ground.  `dolly` != 0: the camera moves that far towards the statue over the
     shutter interval (motion blur).  `extra_light`: None, "point" or "goniometric" -- one more light at the same place above the statue
     (the goniometric one turned, with gonio_map()): what the image lookup of a goniometric light costs.  `camera`: "perspective",
-    "orthographic" (a view 3.2 units high either side of the axis) or "environment" (the whole sphere around the same eye)."""
+    "orthographic" (a view 3.2 units high either side of the axis), "environment" (the whole sphere around the same eye) or "realistic"
+    (DGAUSS_50MM on a 35 mm film, focused on the statue's centre, `aperturediameter` mm)."""
     rng = np.random.default_rng(seed)
     h = HostScene()
     body = h.material(_abi.MAT_MATTE, [0.62, 0.47, 0.33, 0.0])
@@ -500,6 +515,8 @@ def statue(n_side=1468, xres=1024, yres=1024, spp=128, maxdepth=5, seed=1234, wi
         h.camera_orthographic(screenwindow=_screen_window(xres, yres, 3.2))
     elif camera == "environment":
         h.camera_environment()
+    elif camera == "realistic":
+        h.camera_realistic(DGAUSS_50MM, aperturediameter=aperturediameter, focusdistance=float(np.linalg.norm([0.0, 1.2, 7.5])))
     elif camera == "perspective":
         h.camera(fov=38.0)
     else:
