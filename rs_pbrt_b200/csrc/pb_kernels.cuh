@@ -98,7 +98,18 @@ struct BatchInfo {
     uint32_t n_pixels;
     uint32_t first_sample;  // samples [first_sample, first_sample + n_samples) of each pixel
     uint32_t n_samples;
+    uint64_t n_samples_magic;  // div_magic(., n_samples_magic) == . / n_samples (magic_of)
 };
+
+// A camera sample's path state: ray direction, beta = 1, Sobol' index, next dimension 5, for the dense layout of the fields.  The path
+// integrator's interleaved record A is written by k_raygen's tail instead, whole and coalesced (see there).
+PB_D void raygen_state(const DPaths& ps, uint32_t i, V3 d, uint64_t index) {
+    if (ps.path_rec) return;
+    ps.ray_d[i] = make_float4(d.x, d.y, d.z, 0.0f);
+    ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+    ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
+    ps.dim[i] = 5u;
+}
 
 // k_raygen's slot for the realistic camera (integrator.rs:134-160): the camera sample's ray and weight.  A vignetted sample (weight 0)
 // keeps a valid p_film and no PF_HAS_RAY: li does not run (L = 0), and k_resolve<true> still adds its filter weight to the pixel.
@@ -129,42 +140,68 @@ PB_D uint32_t raygen_lens(const DScene& sc, const DRender& rp, DPaths& ps, const
         ps.ray_diff[3 * (size_t)i + 1] = make_float4(ryo.y, ryo.z, rxd.x, rxd.y);
         ps.ray_diff[3 * (size_t)i + 2] = make_float4(rxd.z, ryd.x, ryd.y, ryd.z);
     }
-    ps.ray_d[i] = make_float4(d.x, d.y, d.z, 0.0f);
     ray0 = make_float4(o.x, o.y, o.z, __int_as_float(0x7f800000));
     ray1 = make_float4(d.x, d.y, d.z, __uint_as_float(i | (RAY_EXTEND << 30)));
-    ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+    raygen_state(ps, i, d, index);
     ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(PF_HAS_RAY));
-    ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
-    ps.dim[i] = 5u;
     return 1;
 }
+
+// -----------------------------------------------------------------------------------------------
+// Camera-sample Sobol' tables of one render (Sobol' sampler): 32-byte records {index lo, index hi, raw u32 of dims 0, 1}
+// {raw u32 of dims 2, 3, 4, 0}, for
+//   F[s] = I(s, 0, 0)   s < spp                        records [0, spp)
+//   X[u] = I(0, u, 0)   u < sb[2] - sb[0]              records [spp, spp + wx)
+//   Y[u] = I(0, 0, u)   u < sb[3] - sb[1]              records [spp + wx, spp + wx + wy)
+// where I(s, x, y) = sobol_interval_to_index(m, s, x, y).  Every step of I is linear over GF(2):
+//   I(s, x, y) = (s << 2m) ^ Lvdci(Lvdc(s) ^ (x << m | y)),  Lvdc / Lvdci(b) = XOR of the vdc / vdci rows over the set bits of b,
+// the shifts drop bits past the word as a mask does, and y < 2^m makes x << m | y = (x << m) ^ y, so
+//   I(s, x, y) = I(s, 0, 0) ^ I(0, x, 0) ^ I(0, 0, y).
+// A dimension's raw u32 is the generator matrix applied to the index's first 4 * n_chunks bits, linear again, so it splits the same
+// way.  k_raygen therefore XORs three records where it ran the bit loops of sobol_interval_to_index and five nibble-table walks, and
+// gets the same bits.  The pixel coordinates relative to sb are below the sample bounds' extent (pixels lie in sb), itself <= 2^m.
+__global__ void __launch_bounds__(256) k_camera_sobol(DRender rp, const uint32_t* __restrict__ nib, uint32_t n_chunks, const uint64_t* __restrict__ vdc,
+                                                      const uint64_t* __restrict__ vdci, uint4* __restrict__ tab) {
+    const uint32_t wx = (uint32_t)(rp.sb[2] - rp.sb[0]), wy = (uint32_t)(rp.sb[3] - rp.sb[1]);
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rp.spp + wx + wy) return;
+    uint64_t frame = 0;
+    int u = 0, v = 0;
+    if (i < rp.spp) frame = i;
+    else if (i < rp.spp + wx) u = (int)(i - rp.spp);
+    else v = (int)(i - rp.spp - wx);
+    const uint32_t m = rp.log2_res;  // (m == 0: every index is 0 and the rows are not read)
+    const size_t row = m ? (size_t)(m - 1) * PB_SOBOL_MATRIX_SIZE : 0;
+    SobolCtx sob;
+    sob.nib = nib; sob.stride = PB_SOBOL_CHUNKS; sob.n_chunks = n_chunks; sob.dim = 0; sob.overflow = false;
+    sob.index = sobol_interval_to_index(vdc + row, vdci + row, m, frame, u, v);
+    tab[2 * (size_t)i] = make_uint4((uint32_t)sob.index, (uint32_t)(sob.index >> 32), sobol_sample_nib_u32(sob, 0), sobol_sample_nib_u32(sob, 1));
+    tab[2 * (size_t)i + 1] = make_uint4(sobol_sample_nib_u32(sob, 2), sobol_sample_nib_u32(sob, 3), sobol_sample_nib_u32(sob, 4), 0u);
+}
+PB_D uint4 xor4(uint4 a, uint4 b) { return make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w); }
 
 // -----------------------------------------------------------------------------------------------
 // k_raygen: integrator.rs:123-144, sampler.rs:85-95, sobol.rs:110-138, and the camera's generate_ray_differential
 // (perspective.rs:190-280, orthographic.rs:156-230, environment.rs:92-116).
 // CAM_MOTION: the camera is animated (cam_mo); a static camera's instantiation never reads cam_mo.
 // CAM_KIND: PbrtCameraKind.  env_res: Film.full_resolution as floats, read by the environment camera only.  lens: the realistic
-// camera's lens system, pupil bounds and per-slot weight array, read by that camera only.
+// camera's lens system, pupil bounds and per-slot weight array, read by that camera only.  cam_sobol: this render's k_camera_sobol
+// tables (Sobol' sampler; null for Halton).
 template <bool CAM_MOTION, int CAM_KIND>
-__global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps, BatchInfo bi, const uint32_t* __restrict__ nib, uint32_t n_chunks,
-                                               const uint64_t* __restrict__ vdc, const uint64_t* __restrict__ vdci, uint32_t* __restrict__ queue,
+__global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps, BatchInfo bi, const uint4* __restrict__ cam_sobol, uint32_t* __restrict__ queue,
                                                uint32_t* __restrict__ d_count, float4* __restrict__ rays, uint32_t* __restrict__ d_nrays,
                                                DCounters* cnt, const DMotion cam_mo, const float2 env_res, const DLens lens) {
     constexpr bool ORTHO = CAM_KIND == PBRT_CAMERA_ORTHOGRAPHIC, ENV = CAM_KIND == PBRT_CAMERA_ENVIRONMENT, REAL = CAM_KIND == PBRT_CAMERA_REALISTIC;
-    __shared__ uint64_t s_vdc[52], s_vdci[52];
-    if (threadIdx.x < 52) {
-        uint32_t m = rp.log2_res;
-        s_vdc[threadIdx.x] = m ? vdc[(m - 1) * 52 + threadIdx.x] : 0;
-        s_vdci[threadIdx.x] = m ? vdci[(m - 1) * 52 + threadIdx.x] : 0;
-    }
-    __syncthreads();
+    __shared__ uint32_t s_warp[8], s_base;  // the CTA's ray append (blockDim.x == 256)
+    __shared__ float4 s_ray[256 * 2], s_rec[256 * 4];  // the CTA's rays and records A, staged for coalesced stores
     uint32_t n = bi.n_pixels * bi.n_samples;
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) *d_count = n;
     uint32_t my_rays = 0;
     float4 ray0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), ray1 = ray0;
+    uint64_t ray_index = 0;  // the Sobol' / Halton index of the sample whose ray this thread made
     if (i < n) {
-        uint32_t pl = i / bi.n_samples, s = bi.first_sample + i % bi.n_samples;
+        const uint32_t pl = div_magic(i, bi.n_samples_magic), s = bi.first_sample + (i - pl * bi.n_samples);
         uint32_t pix = bi.first_pixel + pl;
         int px, py;
         const bool in_frame = share_pixel(rp, pix, px, py);
@@ -184,23 +221,27 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
                 ly = halton_sample_dimension(rp, index, 4u);
                 lx = halton_sample_dimension(rp, index, 3u);
             } else {
-                index = sobol_interval_to_index(s_vdc, s_vdci, rp.log2_res, (uint64_t)s, px - rp.sb[0], py - rp.sb[1]);
-                // dims 0,1: film offset remapped to the pixel and clamped (sobol.rs:127-138); y is drawn first
-                SobolCtx sob;
-                sob.nib = nib; sob.stride = PB_SOBOL_CHUNKS; sob.n_chunks = n_chunks; sob.index = index; sob.dim = 0; sob.overflow = false;
-                sy = sobol_sample_nib(sob, 1);
-                sx = sobol_sample_nib(sob, 0);
+                // index and raw dims 0..4 = F[s] ^ X[px - sb0] ^ Y[py - sb1] (k_camera_sobol)
+                const uint4* f = cam_sobol + 2 * (size_t)s;
+                const uint4* xr = cam_sobol + 2 * ((size_t)rp.spp + (uint32_t)(px - rp.sb[0]));
+                const uint4* yr = cam_sobol + 2 * ((size_t)rp.spp + (uint32_t)(rp.sb[2] - rp.sb[0]) + (uint32_t)(py - rp.sb[1]));
+                const uint4 a = xor4(xor4(__ldg(f), __ldg(xr)), __ldg(yr)), b = xor4(xor4(__ldg(f + 1), __ldg(xr + 1)), __ldg(yr + 1));
+                index = (uint64_t)a.x | ((uint64_t)a.y << 32);
+                // dims 0,1: film offset remapped to the pixel and clamped (sobol.rs:127-138)
+                sx = sobol_to_float(a.z);
+                sy = sobol_to_float(a.w);
                 sx = sx * (float)rp.resolution + (float)rp.sb[0];
                 sx = clampf(sx - (float)px, 0.0f, PB_ONE_MINUS_EPSILON);
                 sy = sy * (float)rp.resolution + (float)rp.sb[1];
                 sy = clampf(sy - (float)py, 0.0f, PB_ONE_MINUS_EPSILON);
-                time = sobol_sample_nib(sob, 2);
-                ly = sobol_sample_nib(sob, 4);
-                lx = sobol_sample_nib(sob, 3);
+                time = sobol_to_float(b.x);
+                lx = sobol_to_float(b.y);
+                ly = sobol_to_float(b.z);
             }
             float2 p_film = make_float2((float)px + sx, (float)py + sy);
             if constexpr (REAL) {  // realistic.rs:693-735 (pb_lens.cuh)
                 my_rays = raygen_lens<CAM_MOTION>(sc, rp, ps, lens, cam_mo, i, index, p_film, time, make_float2(lx, ly), ray0, ray1);
+                ray_index = index;
             } else {
                 // raster -> camera (Transform::transform_point transform.rs:490-517)
                 const float* m = sc.raster_to_camera;
@@ -296,22 +337,52 @@ __global__ void __launch_bounds__(256) k_raygen(DScene sc, DRender rp, DPaths ps
                     ps.ray_diff[3 * (size_t)i + 1] = make_float4(ryo.y, ryo.z, rxd.x, rxd.y);
                     ps.ray_diff[3 * (size_t)i + 2] = make_float4(rxd.z, ryd.x, ryd.y, ryd.z);
                 }
-                ps.ray_d[i] = make_float4(dw.x, dw.y, dw.z, 0.0f);
                 ray0 = make_float4(ow.x, ow.y, ow.z, __int_as_float(0x7f800000));  // t_max = inf - dt = inf
                 ray1 = make_float4(dw.x, dw.y, dw.z, __uint_as_float(i | (RAY_EXTEND << 30)));
-                ps.beta[i] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+                raygen_state(ps, i, dw, index);
                 ps.L[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(PF_HAS_RAY));
-                ps.sobol[i] = make_uint2((uint32_t)index, (uint32_t)(index >> 32));
-                ps.dim[i] = 5u;
                 ps.p_film[i] = p_film;
                 my_rays = 1;
+                ray_index = index;
             }
         }
     }
-    uint32_t pos = queue_append(d_nrays, my_rays != 0);  // *d_nrays is zeroed by the host before the launch
-    if (my_rays) { rays[2 * (size_t)pos] = ray0; rays[2 * (size_t)pos + 1] = ray1; }
-    uint32_t tot = warp_sum(my_rays);
-    if ((threadIdx.x & 31) == 0 && tot) atomicAdd(&cnt->camera_rays, (unsigned long long)tot);
+    // One append per CTA: a ray's place in the queue is not observable in the results.  A warp's rays are contiguous in the queue and
+    // its 32 records A in the path state, so both are staged in shared memory and stored 512 contiguous bytes per instruction rather
+    // than one 16-byte piece of a different record per lane.  Record A is written whole, its unused first 16 bytes and last word
+    // included: the L2 writes back a partly written 32-byte sector only after reading the rest of it from HBM.  (A slot without a ray
+    // gets a record too; nothing reads it.)
+    const unsigned bal = __ballot_sync(0xffffffffu, my_rays != 0);
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    if (lane == 0) s_warp[warp] = (uint32_t)__popc(bal);
+    if (my_rays) {
+        const uint32_t k = 2u * (32u * warp + (uint32_t)__popc(bal & ((1u << lane) - 1u)));
+        s_ray[k] = ray0;
+        s_ray[k + 1] = ray1;
+    }
+    if (ps.path_rec) {
+        const float4 z = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        float4* r = s_rec + 4 * threadIdx.x;
+        r[0] = z;
+        r[1] = my_rays ? make_float4(ray1.x, ray1.y, ray1.z, 0.0f) : z;
+        r[2] = make_float4(1.0f, 1.0f, 1.0f, 1.0f);
+        r[3] = my_rays ? make_float4(__uint_as_float((uint32_t)ray_index), __uint_as_float((uint32_t)(ray_index >> 32)), __uint_as_float(5u), 0.0f) : z;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t tot = 0;
+        for (int w = 0; w < 8; ++w) { const uint32_t c = s_warp[w]; s_warp[w] = tot; tot += c; }
+        s_base = tot ? atomicAdd(d_nrays, tot) : 0u;  // *d_nrays is zeroed by the host before the launch
+        if (tot) atomicAdd(&cnt->camera_rays, (unsigned long long)tot);
+    }
+    __syncthreads();
+    const size_t wpos = s_base + s_warp[warp];
+    for (uint32_t k = lane; k < 2u * (uint32_t)__popc(bal); k += 32u) rays[2 * wpos + k] = s_ray[64u * warp + k];
+    if (ps.path_rec) {
+        const uint32_t first = blockIdx.x * blockDim.x + 32u * warp;  // this warp's first slot
+        for (uint32_t k = lane; k < 128u; k += 32u)
+            if (first + (k >> 2) < n) ps.path_rec[4 * (size_t)first + k] = s_rec[128u * warp + k];
+    }
 }
 
 // -----------------------------------------------------------------------------------------------

@@ -128,6 +128,17 @@ PB_HD int f2i_sat(float x) {
     return (int)x;
 #endif
 }
+// Division by a divisor the host knows: magic_of(d) = ceil(2^64 / d) for d >= 2, and div_magic(n, magic_of(d)) == n / d for every n < 2^32
+// (the rounding error n * (magic - 2^64 / d) / 2^64 < 2^-32 stays below the 1 / d that n / d lies below the next integer).  d == 1: magic 0.
+PB_HD uint64_t magic_of(uint32_t d) { return d >= 2u ? ~0ull / d + 1ull : 0ull; }
+PB_HD uint32_t div_magic(uint32_t n, uint64_t magic) {
+    if (!magic) return n;
+#ifdef __CUDA_ARCH__
+    return (uint32_t)__umul64hi((unsigned long long)n, (unsigned long long)magic);
+#else
+    return (uint32_t)(((unsigned __int128)n * magic) >> 64);
+#endif
+}
 PB_HD float clampf(float v, float lo, float hi) { return v < lo ? lo : (v > hi ? hi : v); }  // pbrt.rs:108-121
 PB_HD float lerpf(float t, float a, float b) { return a * (1.0f - t) + b * t; }              // pbrt.rs:235-245
 

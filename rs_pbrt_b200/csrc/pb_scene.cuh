@@ -212,6 +212,7 @@ struct DPaths {
     float4* ray_diff;
     DMaterial* slot_mat;
     float4* slot_frame;  // bump-mapped hits: {shading.n, -} {shading.dpdu, -} per slot
+    float4* path_rec;    // the path integrator's interleaved record A (ray_d, beta, sobol and dim are views into it); null: dense fields
 };
 // bits of L.w
 enum { PF_HAS_RAY = 1u, PF_HAS_SHADOW = 2u, PF_HAS_MIS = 4u, PF_SPECULAR_BOUNCE = 8u, PF_BOUNCES_SHIFT = 8 };
@@ -228,6 +229,7 @@ struct DRender {
     // `pix` of the share is pixel (pix & 15, (pix >> 4) & 15) of tile pix >> 8.  nullptr: the share is `rect`, row-major.
     const uint32_t* tiles;
     uint32_t n_tiles;
+    uint64_t rect_w_magic;        // magic_of(rect[2] - rect[0]): share_pixel's row of a pixel number
     float filter_radius[2];
     float max_sample_luminance;
     uint32_t spp, max_depth;
@@ -251,9 +253,9 @@ PB_D bool share_pixel(const DRender& rp, uint32_t pix, int& px, int& py) {
         py = rp.sb[1] + (int)((t >> 16) << 4) + (int)((pix >> 4) & 15u);
         return px < rp.sb[2] && py < rp.sb[3];
     }
-    const int rw = rp.rect[2] - rp.rect[0];
-    px = rp.rect[0] + (int)(pix % (uint32_t)rw);
-    py = rp.rect[1] + (int)(pix / (uint32_t)rw);
+    const uint32_t rw = (uint32_t)(rp.rect[2] - rp.rect[0]), row = div_magic(pix, rp.rect_w_magic);
+    px = rp.rect[0] + (int)(pix - row * rw);
+    py = rp.rect[1] + (int)row;
     return true;
 }
 

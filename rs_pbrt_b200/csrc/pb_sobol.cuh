@@ -54,15 +54,18 @@ struct SobolCtx {
     uint32_t dim;          // next dimension
     bool overflow;         // the reference panics past 1024 dimensions (sobol.rs:119-124); we flag
 };
-PB_D float sobol_sample_nib(const SobolCtx& s, uint32_t dim) {
+PB_D float sobol_to_float(uint32_t v) { return fminf(__uint2float_rn(v) * 2.3283064365386963e-10f, PB_ONE_MINUS_EPSILON); }
+// the raw u32 of dimension `dim` (before sobol_to_float)
+PB_D uint32_t sobol_sample_nib_u32(const SobolCtx& s, uint32_t dim) {
     const uint32_t* t = s.nib + (size_t)dim * s.stride * 16u;
     uint32_t lo = (uint32_t)s.index, hi = (uint32_t)(s.index >> 32);
     uint32_t v = 0;
     const uint32_t n_lo = s.n_chunks < 8u ? s.n_chunks : 8u;
     for (uint32_t c = 0; c < n_lo; ++c) { v ^= t[c * 16u + (lo & 15u)]; lo >>= 4; }
     for (uint32_t c = 8; c < s.n_chunks; ++c) { v ^= t[c * 16u + (hi & 15u)]; hi >>= 4; }
-    return fminf(__uint2float_rn(v) * 2.3283064365386963e-10f, PB_ONE_MINUS_EPSILON);
+    return v;
 }
+PB_D float sobol_sample_nib(const SobolCtx& s, uint32_t dim) { return sobol_to_float(sobol_sample_nib_u32(s, dim)); }
 // ---- transposed nibble tables for k_shade: nibT[(chunk * 16 + e) * ds + dim] ------------------------------------------------
 // A path vertex draws up to seven consecutive dimensions of ONE Sobol' index (light choice, u_light, u_scattering, the BSDF
 // sample); with the dimension as the fastest index the nibble of each chunk is extracted once and the seven table words sit
@@ -76,7 +79,6 @@ struct SobolT {
     uint32_t dim;
     bool overflow;
 };
-PB_D float sobol_to_float(uint32_t v) { return fminf(__uint2float_rn(v) * 2.3283064365386963e-10f, PB_ONE_MINUS_EPSILON); }
 template <int N>
 PB_D void sobolT_fill(const SobolT& s, float (&out)[N]) {  // dimensions s.dim .. s.dim+N-1; the table is padded by 8 dimensions
     uint32_t acc[N];

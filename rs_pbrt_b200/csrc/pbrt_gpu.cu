@@ -463,6 +463,7 @@ struct DeviceScratch {
     DevBuf<uint4> h_dims;           // HaltonSampler tables, uploaded on first use
     DevBuf<uint16_t> h_perm;
     DevBuf<uint32_t> nibT;          // per-render transposed Sobol' nibble tables for k_shade
+    DevBuf<uint4> cam_sobol;        // per-render camera-sample Sobol' tables for k_raygen (k_camera_sobol)
     DevBuf<uint32_t> tiles;         // tile-interleaved renders: this share's tile list
     DirectBufs direct;              // DirectLighting / Whitted state (pb_direct.cuh)
     std::vector<uint32_t> h_nibT;
@@ -751,6 +752,19 @@ static decltype(&k_raygen<false, PBRT_CAMERA_PERSPECTIVE>) raygen_kernel(const P
     if (sc->cam_kind == PBRT_CAMERA_ENVIRONMENT) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ENVIRONMENT> : k_raygen<false, PBRT_CAMERA_ENVIRONMENT>;
     if (sc->cam_kind == PBRT_CAMERA_REALISTIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_REALISTIC> : k_raygen<false, PBRT_CAMERA_REALISTIC>;
     return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_PERSPECTIVE> : k_raygen<false, PBRT_CAMERA_PERSPECTIVE>;
+}
+
+// k_raygen's camera-sample Sobol' tables for this render (k_camera_sobol, built with the n_chunks k_raygen would use for the index); null
+// for the Halton sampler
+static cudaError_t camera_sobol(DeviceScratch* scr, const PbrtScene* sc, const DRender& rp, uint32_t n_chunks, cudaStream_t st, const uint4** out) {
+    *out = nullptr;
+    if (rp.halton) return cudaSuccess;
+    const uint32_t n = rp.spp + (uint32_t)(rp.sb[2] - rp.sb[0]) + (uint32_t)(rp.sb[3] - rp.sb[1]);
+    cudaError_t e = scr->cam_sobol.alloc(2 * (size_t)n);
+    if (e != cudaSuccess) return e;
+    k_camera_sobol<<<(n + 255) / 256, 256, 0, st>>>(rp, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, scr->cam_sobol.p);
+    *out = scr->cam_sobol.p;
+    return cudaGetLastError();
 }
 
 // k_raygen's lens argument: the scene's realistic-camera record with this batch context's weight array (unused by other cameras)
@@ -1821,6 +1835,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
     while ((1u << rp.log2_res) < rp.resolution) rp.log2_res++;
     if (rp.log2_res > 25) return fail(PBRT_E_UNSUPPORTED, "sample bounds too large for the Sobol' tables");
     const int rw = rp.rect[2] - rp.rect[0], rh = rp.rect[3] - rp.rect[1];
+    rp.rect_w_magic = magic_of((uint32_t)std::max(rw, 1));
     std::vector<uint32_t> h_tiles;
     if (tiled && rw > 0 && rh > 0) {
         const uint32_t ntx = ((uint32_t)rw + 15u) / 16u, nty = ((uint32_t)rh + 15u) / 16u;
@@ -2014,6 +2029,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         uint32_t log2_spp = 0;
         while ((1u << log2_spp) < rp.spp) log2_spp++;
         const uint32_t raygen_chunks = std::max<uint32_t>(1u, (std::min<uint32_t>(52u, 2u * rp.log2_res + log2_spp) + 3u) / 4u);
+        const uint4* cam_sobol_p = nullptr;
+        CK(camera_sobol(scr, sc, rp, std::max(raygen_chunks, dd.n_chunks), st, &cam_sobol_p));
+        launches += halton ? 0 : 1;
         uint32_t* h_poll = nullptr;
         cudaEvent_t poll_ev[2];
         CK(scr->poll_words(&h_poll));
@@ -2025,11 +2043,12 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
                 bi.first_sample = s0;
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
+                bi.n_samples_magic = magic_of(bi.n_samples);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
                 const auto raygen = raygen_kernel(sc);
-                raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, sc->nib.p, std::max(raygen_chunks, dd.n_chunks), sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count,
-                                                        X.rays.p, d_nrays, sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
+                raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, cam_sobol_p, X.queue[0].p, d_count, X.rays.p, d_nrays, sc->counters.p, sc->cam_mo,
+                                                        sc->env_res, lens_arg(sc, X));
                 launches++;
                 // the recursion's length is decided on the device (the active word = camera samples that still need an iteration).  The
                 // host reads that word poll_lag() iterations late (see there: 0 by default, measured): with a lag of 1 iteration i + 1 is
@@ -2089,6 +2108,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             if (array_samples * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 are outside the GPU path");
         } else if (2u * rp.log2_res + log2_arr > 52u) return fail(PBRT_E_UNSUPPORTED, "Sobol' index beyond 52 bits");
         const uint32_t n_chunks = std::max<uint32_t>(1u, (2u * rp.log2_res + log2_arr + 3u) / 4u);
+        const uint4* cam_sobol_p = nullptr;
+        CK(camera_sobol(scr, sc, rp, n_chunks, st, &cam_sobol_p));
+        launches += halton ? 0 : 1;
         const bool count_work = (p->flags & PBRT_RENDER_COUNT_WORK) != 0;
         const uint64_t total_pixels = share_pixels;
         const size_t CAP = (size_t)1 << (getenv("PB_SIBLING_BATCH_LOG2") ? std::min(24, std::max(4, atoi(getenv("PB_SIBLING_BATCH_LOG2")))) : 22);  // any-hit rays in flight per batch
@@ -2139,11 +2161,12 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
                 bi.first_sample = s0;
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
+                bi.n_samples_magic = magic_of(bi.n_samples);
                 const uint32_t n = bi.n_pixels * bi.n_samples;
                 CK(cudaMemsetAsync(d_nrays, 0, 4, st));
                 const auto raygen = raygen_kernel(sc);
-                raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, d_count, X.rays.p, d_nrays,
-                                                        sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
+                raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, cam_sobol_p, X.queue[0].p, d_count, X.rays.p, d_nrays, sc->counters.p, sc->cam_mo,
+                                                        sc->env_res, lens_arg(sc, X));
                 launches++;
                 int rc = trace();
                 if (rc != PBRT_OK) return rc;
@@ -2305,6 +2328,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         const uint32_t sobol_cfg = sobol_ds | (stage_sobol ? 0x80000000u : 0u);
         const size_t shade_smem = stage_sobol ? (size_t)sobol_ds * n_chunks * 64 : 0;
         const uint32_t* shade_nib = scr->nibT.p;
+        const uint4* cam_sobol_p = nullptr;  // (on the caller's stream, ahead of ev_start: every context's k_raygen reads it)
+        CK(camera_sobol(scr, sc, rp, n_chunks, st, &cam_sobol_p));
+        launches += halton ? 0 : 1;
         // persistent trace grid: the CTAs that are resident at once (half of them per stream when two batches overlap)
         const bool instanced = sc->d.n_instances > 0;
         const bool textured = sc->d.n_textures > 0;
@@ -2387,7 +2413,9 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 ps.ld_light = f4(B, 0); ps.mis_d = f4(B, 1); ps.mis_f = f4(B, 2); ps.nee_beta = f4(B, 3);
                 ps.hit = f4(C, 0); ps.mis_hit = f4(C, 1);
                 ps.occl.p = reinterpret_cast<uint32_t*>(C + 2); ps.occl.stride = 16;
+                ps.path_rec = A;
             } else {
+                ps.path_rec = nullptr;
                 ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
                 ps.ld_light = dense_view(X.f4[4].p); ps.mis_hit = dense_view(X.f4[5].p); ps.mis_d = dense_view(X.f4[6].p); ps.mis_f = dense_view(X.f4[7].p);
                 ps.nee_beta = dense_view(X.f4[8].p);
@@ -2545,8 +2573,8 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
             CK(cudaMemsetAsync(V.d_nrays, 0, (5 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
             if (spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
             const auto raygen = raygen_kernel(sc);
-            raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays,
-                                                      sc->counters.p, sc->cam_mo, sc->env_res, lens_arg(sc, X));
+            raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, cam_sobol_p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays, sc->counters.p, sc->cam_mo,
+                                                      sc->env_res, lens_arg(sc, X));
             launches++;
             return PBRT_OK;
         };
@@ -2567,6 +2595,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
                 bi.first_sample = s0;
                 bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
+                bi.n_samples_magic = magic_of(bi.n_samples);
                 batches.push_back(bi);
             }
         const uint32_t iters = rp.max_depth + 1;
