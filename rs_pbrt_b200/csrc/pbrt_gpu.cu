@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -501,17 +502,7 @@ struct DeviceScratch {
         if (e == cudaSuccess) h_film_n = n;
         return e;
     }
-    // loops whose length is only known on the device (null-surface paths, the DirectLighting / Whitted recursion) read their "work
-    // left" word through these pinned slots one iteration late, so the device always has the next iteration queued
-    uint32_t* h_poll = nullptr;
-    cudaError_t poll_words(uint32_t** p) {
-        if (!h_poll) {
-            cudaError_t e = cudaHostAlloc((void**)&h_poll, 16 * sizeof(uint32_t), cudaHostAllocDefault);
-            if (e != cudaSuccess) return e;
-        }
-        *p = h_poll;
-        return cudaSuccess;
-    }
+    uint32_t* h_poll = nullptr;  // LatePoll's pinned slots
     std::vector<cudaEvent_t> ev_pool;
     size_t ev_used = 0;
     cudaError_t event(cudaEvent_t* e) {
@@ -526,14 +517,6 @@ struct DeviceScratch {
     }
     std::mutex mu;
 };
-// bytes one stream context may spend on the spatial light distribution's voxel tables before they go sparse
-static size_t lightgrid_budget() {
-    if (const char* e = std::getenv("PB_LIGHTGRID_BYTES")) {
-        const long long v = std::atoll(e);
-        if (v > 0) return (size_t)v;
-    }
-    return (size_t)4 << 30;
-}
 static DeviceScratch* scratch_for(int device) {
     static DeviceScratch* pool[64] = {nullptr};
     static std::mutex pool_mu;
@@ -585,42 +568,95 @@ struct PbrtScene {
     }
 };
 
+// The render path's environment switches, read in one place.  The experiments' A/B switches and PB_TIMING are read once per process
+// (at its first render call); the test hooks that change batch and table sizes in-process, the poll lag, the tile run and the wide
+// walk length at every call.
+struct Knobs {
+    bool timing;             // PB_TIMING=1: host wall-clock of the phases of one render call on stderr (what a frame costs besides its kernels)
+    int batch_log2;          // PB_BATCH_LOG2 (10..26): path-integrator camera samples per batch; 0 = by scene
+    int shade_spec;          // PB_SHADE_SPEC=0: no single-lobe k_shade instantiations (every class runs the general one); =1: only the Lambert one
+    bool single_stream;      // PB_SINGLE_STREAM=1: one batch in flight
+    int streams;             // PB_STREAMS (1..4): batches in flight; 1 keeps one, >= 2 forces several; 0 = unset
+    // PB_RAY_SORT=1 switches the coherence order of the ray queues on (2: two-level scatter).  It shortens k_trace on Cornell and the
+    // conference scene (not on the 4.3 M-triangle statue), but the three bucketing kernels cost more than that (they re-read the 32 B ray
+    // records and fight over a few hot histogram bins), so it is OFF by default until the keys are produced by k_shade and the histogram
+    // is warp-aggregated (DESIGN.md section 9).
+    int ray_sort;
+    bool state_aos;          // PB_STATE_AOS=0: one dense array per state field instead of the three interleaved records (A/B switch)
+    bool ray_prep;           // PB_RAY_PREP=1: k_rayprep computes the per-ray traversal constants ahead of k_trace (experiment, see pb_kernels.cuh)
+    uint32_t ray_key_mask;   // PB_RAY_KEY_MASK
+    bool wide;               // PB_WIDE=0: A/B switch back to the reference-layout traversal for the scenes that have wide records
+    bool wide_spec;          // PB_WIDE_SPEC=1: the wide traversal with one leaf of look-ahead per lane (pb_trace.cuh::trace_rays_wide_spec)
+    // read at every call
+    int sibling_batch_log2;  // PB_SIBLING_BATCH_LOG2 (4..24): light samples / any-hit rays in flight per direct / AO batch (a test hook that
+                             // forces many small batches); 0 = the integrator's default
+    size_t lightgrid_bytes;  // PB_LIGHTGRID_BYTES: bytes one stream context may spend on the spatial light distribution's voxel tables
+                             // before they go sparse
+    // PB_POLL_LAG (0 / 1): how many iterations late the host reads the "work left" word of a loop whose length only the device knows.
+    // 0 = after every iteration (a stream sync per iteration); 1 = the next iteration is queued before the count of the current one is
+    // read, and an iteration queued past the end returns at once.  On the directlighting and whitted Cornell frames the three empty
+    // launches and two memsets of the extra iteration cost more than the sync they hide, so 0 is the default.
+    uint32_t poll_lag;
+    size_t tile_run;         // PB_TILE_RUN: consecutive Morton tiles dealt to a part at a time
+    int wide_walk;           // PB_WIDE_WALK (1..64): records visited per lane between warp re-synchronisations; 0 = by L2 size
+};
+// (A plain function on purpose: a static local of an inline member function is a GNU-unique symbol, shared by every copy of the
+// library a process loads, which made the A/B harness compare a build with itself.)
+static Knobs knobs() {
+    auto num = [](const char* name, int unset) { const char* e = std::getenv(name); return e ? std::atoi(e) : unset; };
+    auto clamped = [](const char* name, int lo, int hi, int unset) { const char* e = std::getenv(name); return e ? std::min(hi, std::max(lo, std::atoi(e))) : unset; };
+    static const Knobs once = [&] {
+        Knobs k = {};
+        k.timing = num("PB_TIMING", 0) != 0;
+        k.batch_log2 = clamped("PB_BATCH_LOG2", 10, 26, 0);
+        k.shade_spec = num("PB_SHADE_SPEC", 2);
+        k.single_stream = num("PB_SINGLE_STREAM", 0) != 0;
+        k.streams = clamped("PB_STREAMS", 1, 4, 0);
+        k.ray_sort = num("PB_RAY_SORT", 0);
+        k.state_aos = num("PB_STATE_AOS", 1) != 0;
+        k.ray_prep = num("PB_RAY_PREP", 0) != 0;
+        k.ray_key_mask = std::getenv("PB_RAY_KEY_MASK") ? (uint32_t)std::strtoul(std::getenv("PB_RAY_KEY_MASK"), nullptr, 0) : 0x1fffu;
+        k.wide = num("PB_WIDE", 1) != 0;
+        k.wide_spec = num("PB_WIDE_SPEC", 0) != 0;
+        return k;
+    }();
+    Knobs k = once;
+    k.sibling_batch_log2 = clamped("PB_SIBLING_BATCH_LOG2", 4, 24, 0);
+    const char* e = std::getenv("PB_LIGHTGRID_BYTES");
+    k.lightgrid_bytes = e && std::atoll(e) > 0 ? (size_t)std::atoll(e) : (size_t)4 << 30;
+    k.poll_lag = (uint32_t)clamped("PB_POLL_LAG", 0, 1, 0);
+    k.tile_run = (size_t)clamped("PB_TILE_RUN", 1, INT_MAX, 1);
+    k.wide_walk = clamped("PB_WIDE_WALK", 1, 64, 0);
+    return k;
+}
+
 // The k_trace<COUNT, 0, SMEM, INST> variant a render uses, and its persistent grid: object instances take the two-level traversal
 // over global memory, a scene of at most PB_TRACE_SMEM_BYTES is staged in shared memory, anything else walks global memory.
-// PB_WIDE=0: A/B switch back to the reference-layout traversal for the scenes that have wide records.  (A plain function on purpose:
-// a static local of an inline member function is a GNU-unique symbol, shared by every copy of the library a process loads, which
-// made the A/B harness compare a build with itself.)
-static bool wide_enabled() {
-    static const bool on = !(getenv("PB_WIDE") && atoi(getenv("PB_WIDE")) == 0);
-    return on;
-}
-// PB_WIDE_SPEC=1: the wide traversal with one leaf of look-ahead per lane (pb_trace.cuh::trace_rays_wide_spec; scenes without instances)
-static bool wide_spec_enabled() {
-    static const bool on = getenv("PB_WIDE_SPEC") && atoi(getenv("PB_WIDE_SPEC")) != 0;
-    return on;
-}
+using TraceKernel = decltype(&k_trace<false, 0, false>);
 struct TraceLauncher {
     bool count_work = false, inst = false, smem = false, alpha = false, wide = false, wide_spec = false;
     int wide_walk = 16;
     size_t smem_bytes = 0;
-    int grid = 1, blocks_per_sm = 1;
-    // one switch over the instantiations the render paths use (MODE 0): F is called with the kernel's address
-    template <typename F> void with_kernel(F&& f) const {
+    int sm_count = 1, grid = 1, blocks_per_sm = 1;
+    // the instantiation of the render paths' traversal (MODE 0) when the wide records are not used
+    TraceKernel kernel() const {
         if (alpha) {
-            if (inst) { if (count_work) f(k_trace<true, 0, false, true, true>); else f(k_trace<false, 0, false, true, true>); }
-            else { if (count_work) f(k_trace<true, 0, false, false, true>); else f(k_trace<false, 0, false, false, true>); }
-        } else if (inst) { if (count_work) f(k_trace<true, 0, false, true>); else f(k_trace<false, 0, false, true>); }
-        else if (smem) { if (count_work) f(k_trace<true, 0, true>); else f(k_trace<false, 0, true>); }
-        else { if (count_work) f(k_trace<true, 0, false>); else f(k_trace<false, 0, false>); }
+            if (inst) return count_work ? k_trace<true, 0, false, true, true> : k_trace<false, 0, false, true, true>;
+            return count_work ? k_trace<true, 0, false, false, true> : k_trace<false, 0, false, false, true>;
+        }
+        if (inst) return count_work ? k_trace<true, 0, false, true> : k_trace<false, 0, false, true>;
+        if (smem) return count_work ? k_trace<true, 0, true> : k_trace<false, 0, true>;
+        return count_work ? k_trace<true, 0, false> : k_trace<false, 0, false>;
     }
-    cudaError_t init(const PbrtScene* sc, bool count, int sm_count) {
-        count_work = count;
+    cudaError_t init(const PbrtScene* sc, uint32_t render_flags, int sms, const Knobs& K) {
+        count_work = (render_flags & PBRT_RENDER_COUNT_WORK) != 0;
+        sm_count = sms;
         inst = sc->d.n_instances > 0;
         alpha = sc->d.mesh_alpha != nullptr;
         const size_t scene_bytes = (size_t)sc->d.n_nodes * 32 + (size_t)sc->d.n_tris * 48;
         smem = !inst && !alpha && scene_bytes > 0 && scene_bytes <= PB_TRACE_SMEM_BYTES;
         smem_bytes = smem ? scene_bytes : 0;
-        wide = wide_enabled() && sc->d.wide != nullptr && !count_work && !alpha && !smem;
+        wide = K.wide && sc->d.wide != nullptr && !count_work && !alpha && !smem;
         // record visits per lane and round before the warp re-synchronises: long walks keep the lanes that already hold a leaf waiting,
         // which costs more the longer a record fetch takes -- 8 when the records do not fit in L2 (the 4.3 M-triangle statue: 4, 6, 7, 9
         // and 10 were slower on the H100, DESIGN.md §7), 16 when they do (the conference scene); PB_WIDE_WALK overrides
@@ -628,36 +664,26 @@ struct TraceLauncher {
             int l2 = 0;
             cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, sc->device);
             wide_walk = (size_t)sc->d.n_nodes * 64 > (size_t)std::max(l2, 1) ? 8 : 16;
-            if (const char* e_ = getenv("PB_WIDE_WALK")) wide_walk = std::min(64, std::max(1, atoi(e_)));
+            if (K.wide_walk) wide_walk = K.wide_walk;
         }
         int bps = 1;
         cudaError_t e = cudaSuccess;
-        wide_spec = wide && !inst && wide_spec_enabled();
+        wide_spec = wide && !inst && K.wide_spec;
         if (wide_spec) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_trace_wide_spec, PB_TRACE_THREADS, 0);
         else if (wide) e = inst ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_trace_wide_inst, PB_TRACE_THREADS, 0)
                            : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_trace_wide_plain, PB_TRACE_THREADS, 0);
-        else with_kernel([&](auto k) { e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k, PB_TRACE_THREADS, smem_bytes); });
+        else e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kernel(), PB_TRACE_THREADS, smem_bytes);
         blocks_per_sm = bps;
         grid = sm_count * std::max(1, bps);
         return e;
     }
     void launch(const DScene& d, const TraceIO& io, const uint32_t* d_nrays, uint32_t* d_cursor, DCounters* cnt, cudaStream_t s) const {
         if (wide_spec) k_trace_wide_spec<<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, d_cursor, cnt, wide_walk);
-        else if (wide) {
-            if (inst) k_trace_wide_inst<<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, d_cursor, cnt, wide_walk);
-            else k_trace_wide_plain<<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, d_cursor, cnt, wide_walk);
-        } else if (alpha) {
-            if (inst) { if (count_work) k_trace<true, 0, false, true, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt); else k_trace<false, 0, false, true, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt); }
-            else { if (count_work) k_trace<true, 0, false, false, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt); else k_trace<false, 0, false, false, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt); }
-        } else if (inst) {
-            if (count_work) k_trace<true, 0, false, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
-            else k_trace<false, 0, false, true><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
-        } else if (smem) {
-            if (count_work) k_trace<true, 0, true><<<grid, PB_TRACE_THREADS, smem_bytes, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
-            else k_trace<false, 0, true><<<grid, PB_TRACE_THREADS, smem_bytes, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
-        } else {
-            if (count_work) k_trace<true, 0, false><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
-            else k_trace<false, 0, false><<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
+        else if (wide && inst) k_trace_wide_inst<<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, d_cursor, cnt, wide_walk);
+        else if (wide) k_trace_wide_plain<<<grid, PB_TRACE_THREADS, 0, s>>>(d, io, d_nrays, d_cursor, cnt, wide_walk);
+        else {
+            const TraceKernel k = kernel();
+            k<<<grid, PB_TRACE_THREADS, smem_bytes, s>>>(d, io, d_nrays, 0, d_cursor, cnt);
         }
     }
 };
@@ -745,36 +771,6 @@ static bool enable_peer_access(int from, int to) {
     cudaGetLastError();
     return e == cudaErrorPeerAccessAlreadyEnabled;
 }
-
-// k_raygen's instantiation for a scene's camera: its kind, animated or not
-static decltype(&k_raygen<false, PBRT_CAMERA_PERSPECTIVE>) raygen_kernel(const PbrtScene* sc) {
-    if (sc->cam_kind == PBRT_CAMERA_ORTHOGRAPHIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ORTHOGRAPHIC> : k_raygen<false, PBRT_CAMERA_ORTHOGRAPHIC>;
-    if (sc->cam_kind == PBRT_CAMERA_ENVIRONMENT) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ENVIRONMENT> : k_raygen<false, PBRT_CAMERA_ENVIRONMENT>;
-    if (sc->cam_kind == PBRT_CAMERA_REALISTIC) return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_REALISTIC> : k_raygen<false, PBRT_CAMERA_REALISTIC>;
-    return sc->cam_motion ? k_raygen<true, PBRT_CAMERA_PERSPECTIVE> : k_raygen<false, PBRT_CAMERA_PERSPECTIVE>;
-}
-
-// k_raygen's camera-sample Sobol' tables for this render (k_camera_sobol, built with the n_chunks k_raygen would use for the index); null
-// for the Halton sampler
-static cudaError_t camera_sobol(DeviceScratch* scr, const PbrtScene* sc, const DRender& rp, uint32_t n_chunks, cudaStream_t st, const uint4** out) {
-    *out = nullptr;
-    if (rp.halton) return cudaSuccess;
-    const uint32_t n = rp.spp + (uint32_t)(rp.sb[2] - rp.sb[0]) + (uint32_t)(rp.sb[3] - rp.sb[1]);
-    cudaError_t e = scr->cam_sobol.alloc(2 * (size_t)n);
-    if (e != cudaSuccess) return e;
-    k_camera_sobol<<<(n + 255) / 256, 256, 0, st>>>(rp, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, scr->cam_sobol.p);
-    *out = scr->cam_sobol.p;
-    return cudaGetLastError();
-}
-
-// k_raygen's lens argument: the scene's realistic-camera record with this batch context's weight array (unused by other cameras)
-static DLens lens_arg(const PbrtScene* sc, const BatchCtx& X) {
-    DLens L = sc->lens;
-    L.weight = X.cam_weight.p;
-    return L;
-}
-// k_resolve's instantiation: the realistic camera's samples carry a weight, every other camera's weight is 1
-static decltype(&k_resolve<false>) resolve_kernel(const PbrtScene* sc) { return sc->cam_kind == PBRT_CAMERA_REALISTIC ? k_resolve<true> : k_resolve<false>; }
 
 // ---- scene creation --------------------------------------------------------------------------------------------------------------
 // pbrt_gpu_scene_create, _create_motion and _create_multi are one code path in two phases.  scene_prepare validates the description
@@ -1778,18 +1774,6 @@ struct Share {
     const int32_t* rect = nullptr;
     uint32_t part = 0, n_parts = 0;
 };
-// Loops whose length only the device knows (the DirectLighting / Whitted recursion, path renders through null surfaces): how many
-// iterations late the host reads the "work left" word.  0 = after every iteration (a stream sync per iteration); 1 = the next iteration is
-// queued before the count of the current one is read, and an iteration queued past the end returns at once.  On the directlighting and
-// whitted Cornell frames the three empty launches and two memsets of the extra iteration cost more than the sync they hide, so 0 is the default.
-static uint32_t poll_lag() {
-    if (const char* e = std::getenv("PB_POLL_LAG")) return (uint32_t)std::min(1, std::max(0, atoi(e)));
-    return 0u;
-}
-static size_t tile_run() {
-    if (const char* e = std::getenv("PB_TILE_RUN")) return (size_t)std::max(1, atoi(e));
-    return 1;
-}
 static uint32_t morton2(uint32_t x, uint32_t y) {  // blockqueue/mod.rs morton2: interleave the low 16 bits of x and y
     auto spread = [](uint32_t v) {
         v &= 0xffffu;
@@ -1801,27 +1785,50 @@ static uint32_t morton2(uint32_t x, uint32_t y) {  // blockqueue/mod.rs morton2:
     };
     return spread(x) | (spread(y) << 1);
 }
-static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& share, float* d_film, float* d_samples, cudaStream_t st,
-                       PbrtStats* stats) {
-    const bool tiled = share.n_parts > 0;
-    const int32_t* rect_in = tiled ? (p ? p->sample_bounds : nullptr) : share.rect;
-    if (!sc || !p || !rect_in) return fail(PBRT_E_INVALID, "null argument");
-    if (tiled && share.part >= share.n_parts) return fail(PBRT_E_INVALID, "tile share out of range");
-    if (tiled && d_samples) return fail(PBRT_E_INVALID, "per-sample output needs a pixel rectangle");
-    // PB_TIMING=1: host wall-clock of the phases of one render call on stderr (what a frame costs besides its kernels)
-    static const bool timing = getenv("PB_TIMING") && atoi(getenv("PB_TIMING"));
-    const auto t_enter = std::chrono::steady_clock::now();
-    auto since = [&](const char* what) {
-        if (timing) fprintf(stderr, "[pb timing] dev %d %-28s %8.3f ms\n", sc->device, what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enter).count());
-    };
-    CK(cudaSetDevice(sc->device));
+
+// One render call as the integrators see it: the caller's parameters, film and stream, the prepared DRender, and the launch and event
+// accounting that PbrtStats reports (ms_trace / ms_shade sum the event pairs in tev / sev).
+struct RenderCall {
+    const PbrtRenderParams* p = nullptr;
+    DRender rp;
+    uint64_t share_pixels = 0;
+    float *d_film = nullptr, *d_samples = nullptr;
+    cudaStream_t st = nullptr;
+    Knobs knobs;
+    int device = 0;
+    std::chrono::steady_clock::time_point t_enter;
+    cudaEvent_t ev1 = nullptr;  // the end of the frame on st
+    uint32_t launches = 0, trace_launches = 0;
+    std::vector<cudaEvent_t> tev, sev;
+    void since(const char* what) const {
+        if (knobs.timing) fprintf(stderr, "[pb timing] dev %d %-28s %8.3f ms\n", device, what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enter).count());
+    }
+};
+#define TRY(call)                             \
+    do {                                      \
+        const int rc_ = (call);               \
+        if (rc_ != PBRT_OK) return rc_;       \
+    } while (0)
+
+// k_texture, k_direct_step and the alpha test keep a DMaterial (and a texture-graph stack) in local memory: stack frames of ~1.5 KB, above
+// the default per-thread stack limit of 1 KB.  Raised once per device (a no-op if the driver sizes known frames by itself).
+static int raise_stack_limit() {
+    size_t cur = 0;
+    CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
+    if (cur < 4096) CK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
+    return PBRT_OK;
+}
+
+// Validates the parameters and fills R.rp (without the sampler tables) and the share: its tile list and pixel count
+static int render_setup(const PbrtScene* sc, const PbrtRenderParams* p, const Share& share, const int32_t* rect_in, RenderCall& R,
+                        std::vector<uint32_t>& h_tiles) {
     if (p->sampler > PBRT_SAMPLER_HALTON) return fail(PBRT_E_UNSUPPORTED, "sampler outside the GPU path");
     const bool halton = p->sampler == PBRT_SAMPLER_HALTON;
     if (p->spp == 0) return fail(PBRT_E_INVALID, "spp must be positive");
     if (!halton && (p->spp & (p->spp - 1)) != 0) return fail(PBRT_E_INVALID, "spp must be a power of two (SobolSampler rounds up, sobol.rs:39-45)");
     if (!(p->filter_radius[0] > 0.0f) || !(p->filter_radius[1] > 0.0f)) return fail(PBRT_E_INVALID, "filter radius must be positive");
     if (p->light_strategy > 2) return fail(PBRT_E_INVALID, "unknown light strategy");
-    DRender rp;
+    DRender& rp = R.rp;
     std::memset(&rp, 0, sizeof rp);
     for (int i = 0; i < 4; ++i) { rp.sb[i] = p->sample_bounds[i]; rp.cb[i] = p->cropped_pixel_bounds[i]; rp.pb[i] = p->pixel_bounds[i]; rp.rect[i] = rect_in[i]; }
     if (rp.rect[0] < rp.sb[0] || rp.rect[1] < rp.sb[1] || rp.rect[2] > rp.sb[2] || rp.rect[3] > rp.sb[3]) return fail(PBRT_E_INVALID, "pixel_rect outside sample_bounds");
@@ -1836,7 +1843,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
     if (rp.log2_res > 25) return fail(PBRT_E_UNSUPPORTED, "sample bounds too large for the Sobol' tables");
     const int rw = rp.rect[2] - rp.rect[0], rh = rp.rect[3] - rp.rect[1];
     rp.rect_w_magic = magic_of((uint32_t)std::max(rw, 1));
-    std::vector<uint32_t> h_tiles;
+    const bool tiled = share.n_parts > 0;
     if (tiled && rw > 0 && rh > 0) {
         const uint32_t ntx = ((uint32_t)rw + 15u) / 16u, nty = ((uint32_t)rh + 15u) / 16u;
         if (ntx > 0xffffu || nty > 0xffffu) return fail(PBRT_E_UNSUPPORTED, "frame larger than 65535 tiles on a side");
@@ -1844,824 +1851,826 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         for (uint32_t ty = 0; ty < nty; ++ty)
             for (uint32_t tx = 0; tx < ntx; ++tx) order[(size_t)ty * ntx + tx] = {morton2(tx, ty), tx | (ty << 16)};
         std::sort(order.begin(), order.end());
-        const size_t run = tile_run();  // consecutive Morton tiles dealt to a part at a time
         for (size_t i = 0; i < order.size(); ++i)
-            if ((i / run) % share.n_parts == share.part) h_tiles.push_back(order[i].second);
+            if ((i / R.knobs.tile_run) % share.n_parts == share.part) h_tiles.push_back(order[i].second);
     }
-    const uint64_t share_pixels = tiled ? (uint64_t)h_tiles.size() * 256u : (uint64_t)std::max(rw, 0) * (uint64_t)std::max(rh, 0);
-    if (share_pixels >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "more than 2^32 pixels in one render call");
-    const uint32_t nl = sc->d.n_lights;
+    R.share_pixels = tiled ? (uint64_t)h_tiles.size() * 256u : (uint64_t)std::max(rw, 0) * (uint64_t)std::max(rh, 0);
+    if (R.share_pixels >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "more than 2^32 pixels in one render call");
     // effective light strategy (lightdistrib.rs:393-418)
     uint32_t strategy = p->light_strategy;
-    if (strategy == PBRT_LIGHTS_UNIFORM || nl == 1) strategy = PBRT_LIGHTS_UNIFORM;
+    if (strategy == PBRT_LIGHTS_UNIFORM || sc->d.n_lights == 1) strategy = PBRT_LIGHTS_UNIFORM;
     rp.light_strategy = strategy;
+    return PBRT_OK;
+}
+
+// HaltonSampler::new (halton.rs:84-112); the sampler's tables are uploaded on first use
+static int halton_setup(DeviceScratch* scr, const PbrtRenderParams* p, DRender& rp) {
+    rp.halton = 1u;
+    rp.h_center = p->sample_at_pixel_center ? 1u : 0u;
+    const int res[2] = {rp.sb[2] - rp.sb[0], rp.sb[3] - rp.sb[1]};
+    for (int i = 0; i < 2; ++i) {
+        const int base = i == 0 ? 2 : 3;
+        int scale = 1, e = 0;
+        while (scale < std::min(res[i], 128)) { scale *= base; e += 1; }
+        rp.h_scale[i] = (uint32_t)scale;
+        rp.h_exp[i] = (uint32_t)e;
+    }
+    rp.h_stride = rp.h_scale[0] * rp.h_scale[1];
+    rp.h_mult[0] = (uint32_t)halton_mult_inverse(rp.h_scale[1], rp.h_scale[0]);
+    rp.h_mult[1] = (uint32_t)halton_mult_inverse(rp.h_scale[0], rp.h_scale[1]);
+    if ((uint64_t)rp.spp * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 (spp * 128 * 243) are outside the GPU path");
+    const HaltonTables& T = halton_tables();
+    if (!scr->h_dims.p) {
+        CK(scr->h_dims.upload(T.dims));
+        CK(scr->h_perm.upload(T.perms));
+    }
+    rp.h_dims = scr->h_dims.p;
+    rp.h_perm = scr->h_perm.p;
+    return PBRT_OK;
+}
+
+// The frame's end: ev1 behind everything queued on the caller's stream, then wait for it
+static int end_frame(RenderCall& R) {
+    CK(cudaEventRecord(R.ev1, R.st));
+    CK(cudaStreamSynchronize(R.st));
+    return PBRT_OK;
+}
+
+// A frame's camera samples in batches of at most `max_samples`: runs of each pixel's samples (all of them when they fit) over as many
+// pixels as fit; sample runs outer, pixels inner.  `cap` is the largest batch.
+struct BatchPlan {
+    uint32_t samples_per_batch, pixels_per_batch;
+    size_t cap;
+    std::vector<BatchInfo> batches;
+};
+static BatchPlan batch_plan(uint32_t spp, uint64_t pixels, uint32_t max_samples) {
+    BatchPlan B;
+    B.samples_per_batch = std::min(spp, max_samples);
+    B.pixels_per_batch = (uint32_t)std::min<uint64_t>(std::max<uint32_t>(1u, max_samples / B.samples_per_batch), pixels);
+    B.cap = (size_t)B.samples_per_batch * B.pixels_per_batch;
+    for (uint32_t s0 = 0; s0 < spp; s0 += B.samples_per_batch)
+        for (uint64_t pix0 = 0; pix0 < pixels; pix0 += B.pixels_per_batch) {
+            BatchInfo bi;
+            bi.first_pixel = (uint32_t)pix0;
+            bi.n_pixels = (uint32_t)std::min<uint64_t>(B.pixels_per_batch, pixels - pix0);
+            bi.first_sample = s0;
+            bi.n_samples = std::min(B.samples_per_batch, spp - s0);
+            bi.n_samples_magic = magic_of(bi.n_samples);
+            B.batches.push_back(bi);
+        }
+    return B;
+}
+
+static uint32_t ceil_log2(uint64_t n) {
+    uint32_t l = 0;
+    while ((1ull << l) < n) l++;
+    return l;
+}
+// 4-bit chunks of the Sobol' index of pixel sample numbers below `samples`: 2 log2(resolution) pixel bits + log2(samples) sample bits
+// (sobol_interval_to_index), at most 52
+static uint32_t sobol_chunks(const DRender& rp, uint64_t samples) {
+    return std::max<uint32_t>(1u, (std::min<uint32_t>(52u, 2u * rp.log2_res + ceil_log2(samples)) + 3u) / 4u);
+}
+// The direct and AO integrators' 2D sample arrays reach pixel sample number `array_samples`: its index must fit the sampler's
+static int check_array_index(const DRender& rp, uint64_t array_samples) {
+    if (rp.halton) {
+        if (array_samples * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 are outside the GPU path");
+    } else if (2u * rp.log2_res + ceil_log2(array_samples) > 52u) return fail(PBRT_E_UNSUPPORTED, "Sobol' index beyond 52 bits");
+    return PBRT_OK;
+}
+
+static int upload_filter(RenderCall& R, DeviceScratch* scr) {
+    CK(scr->filter_table.alloc(256));
+    CK(cudaMemcpyAsync(scr->filter_table.p, R.p->filter_table, 256 * 4, cudaMemcpyHostToDevice, R.st));
+    return PBRT_OK;
+}
+
+// k_raygen's camera-sample Sobol' tables for this render (k_camera_sobol, built with the n_chunks k_raygen would use for the index); null
+// for the Halton sampler
+static int camera_sobol(RenderCall& R, DeviceScratch* scr, const PbrtScene* sc, uint32_t n_chunks, const uint4** out) {
+    *out = nullptr;
+    const DRender& rp = R.rp;
+    if (rp.halton) return PBRT_OK;
+    const uint32_t n = rp.spp + (uint32_t)(rp.sb[2] - rp.sb[0]) + (uint32_t)(rp.sb[3] - rp.sb[1]);
+    CK(scr->cam_sobol.alloc(2 * (size_t)n));
+    k_camera_sobol<<<(n + 255) / 256, 256, 0, R.st>>>(rp, sc->nib.p, n_chunks, sc->vdc.p, sc->vdci.p, scr->cam_sobol.p);
+    R.launches++;
+    *out = scr->cam_sobol.p;
+    CK(cudaGetLastError());
+    return PBRT_OK;
+}
+
+// One batch's camera rays into batch context X (ray count at X.counts + 3), by k_raygen's instantiation for the scene's camera: its
+// kind, animated or not.  `d` is the scene as the integrator shades it; the lens argument is the scene's realistic-camera record with
+// X's weight array (unused by other cameras).
+static void launch_raygen(RenderCall& R, const PbrtScene* sc, const DScene& d, const DPaths& ps, const BatchInfo& bi, const uint4* cam_sobol, BatchCtx& X,
+                          cudaStream_t s) {
+    auto raygen = sc->cam_motion ? k_raygen<true, PBRT_CAMERA_PERSPECTIVE> : k_raygen<false, PBRT_CAMERA_PERSPECTIVE>;
+    if (sc->cam_kind == PBRT_CAMERA_ORTHOGRAPHIC) raygen = sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ORTHOGRAPHIC> : k_raygen<false, PBRT_CAMERA_ORTHOGRAPHIC>;
+    if (sc->cam_kind == PBRT_CAMERA_ENVIRONMENT) raygen = sc->cam_motion ? k_raygen<true, PBRT_CAMERA_ENVIRONMENT> : k_raygen<false, PBRT_CAMERA_ENVIRONMENT>;
+    if (sc->cam_kind == PBRT_CAMERA_REALISTIC) raygen = sc->cam_motion ? k_raygen<true, PBRT_CAMERA_REALISTIC> : k_raygen<false, PBRT_CAMERA_REALISTIC>;
+    DLens lens = sc->lens;
+    lens.weight = X.cam_weight.p;
+    const uint32_t n = bi.n_pixels * bi.n_samples;
+    raygen<<<(n + 255) / 256, 256, 0, s>>>(d, R.rp, ps, bi, cam_sobol, X.queue[0].p, X.counts.p, X.rays.p, X.counts.p + 3, sc->counters.p, sc->cam_mo, sc->env_res, lens);
+    R.launches++;
+}
+// One batch's samples into the film: the realistic camera's samples carry a weight (k_resolve<true>), every other camera's weight is 1
+static void launch_resolve(RenderCall& R, const PbrtScene* sc, DeviceScratch* scr, const DPaths& ps, const BatchInfo& bi, const BatchCtx& X, cudaStream_t s) {
+    const auto resolve = sc->cam_kind == PBRT_CAMERA_REALISTIC ? k_resolve<true> : k_resolve<false>;
+    resolve<<<(bi.n_pixels + 255) / 256, 256, 0, s>>>(R.rp, ps, bi, scr->filter_table.p, R.d_film, R.d_samples, X.cam_weight.p);
+    R.launches++;
+}
+
+// One k_trace launch (k_rayprep ahead of it when `pre` is given) inside an event pair that ms_trace sums.  `counts` is a batch
+// context's counter block: ray count at + 3, ray cursor at + 4.  The direct and AO loops reset the cursor first; the path integrator's
+// kernels reset it for each other.
+static int trace_step(RenderCall& R, DeviceScratch* scr, const TraceLauncher& tl, const PbrtScene* sc, const DScene& d, TraceIO& io, uint32_t* counts,
+                      cudaStream_t s, bool reset_cursor, float4* pre) {
+    if (reset_cursor) CK(cudaMemsetAsync(counts + 4, 0, 4, s));
+    cudaEvent_t a, b;
+    CK(scr->event(&a)); CK(scr->event(&b));
+    CK(cudaEventRecord(a, s));
+    io.pre = pre;
+    if (pre) {
+        k_rayprep<<<tl.sm_count * 8, 256, 0, s>>>(io.rays, counts + 3, pre);
+        R.launches++;
+    }
+    tl.launch(d, io, counts + 3, counts + 4, sc->counters.p, s);
+    CK(cudaEventRecord(b, s));
+    R.tev.push_back(a); R.tev.push_back(b);
+    R.launches++; R.trace_launches++;
+    return PBRT_OK;
+}
+
+// Loops whose length only the device knows (the DirectLighting / Whitted recursion, path renders through null surfaces) read their
+// "work left" word through pinned slots `lag` iterations late (Knobs::poll_lag): with a lag of 1, iteration i + 1 is already queued when
+// i's word arrives, and the iteration queued past the end sees the previous word at 0 and returns at once.
+struct LatePoll {
+    uint32_t* h = nullptr;
+    cudaEvent_t ev[2];
+    uint32_t lag = 0;
+    int init(DeviceScratch* scr, uint32_t lag_) {
+        if (!scr->h_poll) CK(cudaHostAlloc((void**)&scr->h_poll, 2 * sizeof(uint32_t), cudaHostAllocDefault));
+        h = scr->h_poll;
+        CK(scr->event(&ev[0])); CK(scr->event(&ev[1]));
+        lag = lag_;
+        return PBRT_OK;
+    }
+    // queues the read of iteration `it`'s word; *done: the word of iteration it - lag is 0
+    int poll(uint32_t it, const uint32_t* d_word, cudaStream_t s, bool* done) {
+        CK(cudaMemcpyAsync(&h[it & 1u], d_word, 4, cudaMemcpyDeviceToHost, s));
+        CK(cudaEventRecord(ev[it & 1u], s));
+        *done = false;
+        if (it >= lag) {
+            CK(cudaEventSynchronize(ev[(it - lag) & 1u]));
+            *done = h[(it - lag) & 1u] == 0u;
+        }
+        return PBRT_OK;
+    }
+};
+
+// a kernel asked for a sample dimension beyond the sampler's
+static int fail_dims(const DRender& rp) {
+    return fail(PBRT_E_UNSUPPORTED, rp.halton ? "HaltonSampler can only sample 1000 dimensions (halton.rs:256-262)"
+                                              : "SobolSampler can only sample up to 1024 dimensions (sobol.rs:119-124)");
+}
+
+// The dense camera-sample state of the direct and AO integrators in batch context X (cap samples): ray direction, hit, beta, L,
+// Sobol' state, film position, realistic-camera weight, raygen's queue and the counters
+static int dense_state(const PbrtScene* sc, BatchCtx& X, size_t cap, DPaths& ps) {
+    for (int i = 0; i < 4; ++i) CK(X.f4[i].alloc(cap));
+    CK(X.sobol.alloc(cap)); CK(X.dim.alloc(cap)); CK(X.pfilm.alloc(cap));
+    if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
+    CK(X.queue[0].alloc(cap)); CK(X.counts.alloc(8 + PB_SHADE_CLASSES));
+    std::memset(&ps, 0, sizeof ps);
+    ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
+    ps.sobol = dense_view(X.sobol.p); ps.dim = dense_view(X.dim.p); ps.p_film = X.pfilm.p;
+    return PBRT_OK;
+}
+
+// ---- DirectLightingIntegrator / WhittedIntegrator (pb_direct.cuh): raygen -> trace -> { k_direct_step -> k_direct_nee -> trace }
+// until every camera sample's tree is walked -> k_resolve, one batch at a time on the caller's stream.
+static int render_direct(PbrtScene* sc, DeviceScratch* scr, RenderCall& R) {
+    const PbrtRenderParams* p = R.p;
+    const DRender& rp = R.rp;
+    const cudaStream_t st = R.st;
+    const bool whitted = p->integrator == PBRT_INTEGRATOR_WHITTED;
+    const bool sample_all = !whitted && p->direct_strategy == PBRT_DIRECT_SAMPLE_ALL;
+    const uint32_t nl = sc->d.n_lights;
+    if (rp.max_depth > PB_DIRECT_MAX_DEPTH) return fail(PBRT_E_UNSUPPORTED, "direct / whitted maxdepth beyond 8 is outside the GPU path");
+    std::vector<uint32_t> nee_light, nee_k, light_n(nl), light_q0(nl);
+    uint32_t max_n = 1;
+    for (uint32_t j = 0; j < nl; ++j) {
+        light_n[j] = sample_all ? std::max(1u, sc->h_lights[j].n_samples) : 1u;
+        light_q0[j] = (uint32_t)nee_light.size();
+        max_n = std::max(max_n, light_n[j]);
+        if (sample_all || whitted) for (uint32_t k = 0; k < light_n[j]; ++k) { nee_light.push_back(j); nee_k.push_back(k); }
+    }
+    if (!sample_all && !whitted) { nee_light.assign(1, 0u); nee_k.assign(1, 0u); }
+    if (nee_light.empty()) { nee_light.assign(1, 0u); nee_k.assign(1, 0u); }  // no lights: k_direct_nee never has work
+    const uint32_t n_nee = (uint32_t)nee_light.size();
+    if (n_nee > 4096) return fail(PBRT_E_UNSUPPORTED, "more than 4096 light samples per vertex are outside the GPU path");
+    DDirect dd;
+    std::memset(&dd, 0, sizeof dd);
+    dd.max_depth = rp.max_depth; dd.n_nee = n_nee; dd.whitted = whitted ? 1u : 0u; dd.sample_all = sample_all ? 1u : 0u;
+    dd.n_arrays = sample_all ? 2u * nl * rp.max_depth : 0u;
+    dd.array_end = 5u + 2u * dd.n_arrays;
+    const uint64_t array_samples = (uint64_t)rp.spp * max_n;  // pixel sample numbers the 2D arrays reach
+    TRY(check_array_index(rp, array_samples));
+    dd.n_chunks = sobol_chunks(rp, array_samples);
+    const size_t CAP = (size_t)1 << (R.knobs.sibling_batch_log2 ? R.knobs.sibling_batch_log2 : 21);  // light samples in flight per batch
+    const BatchPlan B = batch_plan(rp.spp, R.share_pixels, (uint32_t)std::max<size_t>(1, std::min<size_t>((size_t)1 << 20, CAP / n_nee)));
+    const size_t cap = B.cap, cap_nee = cap * n_nee, depth_n = std::max(1u, rp.max_depth);
+    dd.cap = cap;
+    TRY(upload_filter(R, scr));
+    BatchCtx& X = scr->ctx[0];
+    DPaths ps;
+    TRY(dense_state(sc, X, cap, ps));
+    CK(X.rays.alloc(2 * (cap + 2 * cap_nee)));
+    DirectBufs& D = scr->direct;
+    const bool dinst = sc->d.n_instances > 0;
+    const bool dtex = sc->d.n_textures > 0;
+    CK(D.u32.alloc(6 * cap + 2 * cap_nee + 2 * (size_t)n_nee + 2 * (size_t)std::max(1u, nl) + (dinst ? cap + cap_nee + depth_n * cap : 0) +
+                   (dtex ? cap + depth_n * cap : 0)));
+    CK(D.f4.alloc(4 * depth_n * cap + 4 * cap_nee + (dtex ? 3 * cap + 3 * depth_n * cap : 0)));
+    uint32_t* u = D.u32.p;
+    dd.state = u; u += cap; dd.depth = reinterpret_cast<int*>(u); u += cap; dd.arr_off = u; u += cap;
+    dd.nee_depth = reinterpret_cast<int*>(u); u += cap; dd.nee_dim = u; u += cap; dd.nee_arr = u; u += cap;
+    // (fresh shares the queue buffer, which this integrator does not use otherwise)
+    dd.fresh = X.queue[0].p;
+    dd.nee_flags = u; u += cap_nee; dd.nee_occl = u; u += cap_nee;
+    uint32_t* t_light = u; u += n_nee; uint32_t* t_k = u; u += n_nee; uint32_t* t_n = u; u += std::max(1u, nl); uint32_t* t_q0 = u; u += std::max(1u, nl);
+    uint32_t *d_hit_inst = nullptr, *d_mis_inst = nullptr;
+    if (dinst) { d_hit_inst = u; u += cap; d_mis_inst = u; u += cap_nee; dd.node_inst = u; u += depth_n * cap; }
+    if (dtex) { dd.cur_has_diff = u; u += cap; dd.node_has_diff = u; u += depth_n * cap; }
+    CK(cudaMemcpyAsync(t_light, nee_light.data(), (size_t)n_nee * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(t_k, nee_k.data(), (size_t)n_nee * 4, cudaMemcpyHostToDevice, st));
+    if (nl) {
+        CK(cudaMemcpyAsync(t_n, light_n.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(t_q0, light_q0.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st));
+    }
+    dd.nee_light = t_light; dd.nee_k = t_k; dd.light_n = t_n; dd.light_q0 = t_q0;
+    float4* f = D.f4.p;
+    dd.node_L = f; f += depth_n * cap; dd.node_mul = f; f += depth_n * cap; dd.node_hit = f; f += depth_n * cap; dd.node_rd = f; f += depth_n * cap;
+    dd.nee_a = f; f += cap_nee; dd.nee_mf = f; f += cap_nee; dd.nee_md = f; f += cap_nee; dd.nee_mis_hit = f; f += cap_nee;
+    if (dtex) { dd.cur_diff = f; f += 3 * cap; dd.node_diff = f; f += 3 * depth_n * cap; }
+    CK(cudaStreamSynchronize(st));  // the tables above come from host vectors that go out of scope with this function
+    ps.hit_inst = d_hit_inst; ps.mis_inst = d_mis_inst;
+    if (dtex) {
+        CK(X.ray_diff.alloc(3 * cap)); CK(X.slot_mat.alloc(cap)); CK(X.slot_frame.alloc(2 * cap));
+        ps.ray_diff = X.ray_diff.p; ps.slot_mat = X.slot_mat.p; ps.slot_frame = X.slot_frame.p;
+    }
+    uint32_t* d_active2 = X.counts.p + 5;  // two words: iteration i counts into word i & 1, iteration i + 1 reads it
+    uint32_t* d_err = X.counts.p + 2;
+    uint32_t* d_nrays = X.counts.p + 3;
+    CK(cudaMemsetAsync(d_err, 0, 4, st));
+    TraceIO io;
+    std::memset(&io, 0, sizeof io);
+    io.rays = X.rays.p; io.hit = ps.hit; io.mis_hit = dense_view(dd.nee_mis_hit); io.occl = dense_view(dd.nee_occl);
+    io.hit_inst = d_hit_inst; io.mis_inst = d_mis_inst; io.instancing = rp.instancing;
+    DScene dsc = sc->d;
+    dsc.materials = sc->materials_single.p;  // allow_multiple_lobes = false
+    TraceLauncher tl;
+    CK(tl.init(sc, R.p->flags, sm_count_of(sc->device), R.knobs));
+    const uint4* cam_sobol_p = nullptr;
+    TRY(camera_sobol(R, scr, sc, dd.n_chunks, &cam_sobol_p));
+    LatePoll poll;
+    TRY(poll.init(scr, R.knobs.poll_lag));
+    for (const BatchInfo& bi : B.batches) {
+        const uint32_t n = bi.n_pixels * bi.n_samples;
+        CK(cudaMemsetAsync(d_nrays, 0, 4, st));
+        launch_raygen(R, sc, dsc, ps, bi, cam_sobol_p, X, st);
+        // the recursion's length is decided on the device (the active word = camera samples that still need an iteration)
+        for (uint32_t iter = 0;; ++iter) {
+            TRY(trace_step(R, scr, tl, sc, dsc, io, X.counts.p, st, true, nullptr));
+            uint32_t* d_active = d_active2 + (iter & 1u);
+            const uint32_t* d_prev = iter ? d_active2 + ((iter - 1u) & 1u) : nullptr;
+            CK(cudaMemsetAsync(d_nrays, 0, 4, st));
+            CK(cudaMemsetAsync(d_active, 0, 4, st));
+            cudaEvent_t e, g;
+            CK(scr->event(&e)); CK(scr->event(&g));
+            CK(cudaEventRecord(e, st));
+            const bool env_start = iter == 0 && sc->cam_kind == PBRT_CAMERA_ENVIRONMENT;  // camera rays without a differential
+            if (env_start) {
+                k_direct_start_nodiff<<<(n + 127) / 128, 128, 0, st>>>(dsc, ps, dd, bi);
+                R.launches++;
+            }
+            k_direct_step<<<(n + 127) / 128, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, iter == 0 && !env_start ? 1u : 0u, X.rays.p, d_nrays, d_active, d_err, d_prev);
+            const uint64_t total = (uint64_t)n * n_nee;
+            const unsigned nee_grid = (unsigned)((total + 127) / 128);
+            if (sc->light_level >= 2) k_direct_nee<2><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
+            else k_direct_nee<1><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
+            CK(cudaEventRecord(g, st));
+            R.sev.push_back(e); R.sev.push_back(g);
+            R.launches += 2;
+            bool done = false;
+            TRY(poll.poll(iter, d_active, st, &done));
+            if (done) break;
+            if (iter > 100000u) return fail(PBRT_E_CUDA, "direct integrator did not terminate");
+        }
+        launch_resolve(R, sc, scr, ps, bi, X, st);
+    }
+    CK(cudaGetLastError());
+    uint32_t h_err = 0;
+    CK(cudaMemcpyAsync(&h_err, d_err, 4, cudaMemcpyDeviceToHost, st));
+    TRY(end_frame(R));
+    return h_err ? fail_dims(rp) : PBRT_OK;
+}
+
+// ---- AOIntegrator (integrators/ao.rs): raygen -> trace -> k_ao_shade (ao_n any-hit rays per camera sample) -> trace -> k_ao_resolve
+// -> k_resolve, one batch at a time on the caller's stream.
+static int render_ao(PbrtScene* sc, DeviceScratch* scr, RenderCall& R) {
+    const PbrtRenderParams* p = R.p;
+    const DRender& rp = R.rp;
+    const cudaStream_t st = R.st;
+    const uint32_t ao_n = p->ao_samples;
+    if (ao_n == 0 || ao_n > 4096) return fail(PBRT_E_INVALID, "ao nsamples out of range (1..4096)");
+    const uint64_t array_samples = (uint64_t)rp.spp * ao_n;  // pixel sample numbers the 2D array reaches
+    TRY(check_array_index(rp, array_samples));
+    const uint32_t n_chunks = sobol_chunks(rp, array_samples);
+    const uint4* cam_sobol_p = nullptr;
+    TRY(camera_sobol(R, scr, sc, n_chunks, &cam_sobol_p));
+    const size_t CAP = (size_t)1 << (R.knobs.sibling_batch_log2 ? R.knobs.sibling_batch_log2 : 22);  // any-hit rays in flight per batch
+    const BatchPlan B = batch_plan(rp.spp, R.share_pixels, (uint32_t)std::max<size_t>(1, CAP / ao_n));
+    const size_t cap_paths = B.cap, cap_rays = cap_paths * ao_n;
+    TRY(upload_filter(R, scr));
+    BatchCtx& X = scr->ctx[0];
+    DPaths ps;
+    TRY(dense_state(sc, X, cap_paths, ps));
+    CK(X.rays.alloc(2 * std::max(cap_paths, cap_rays)));
+    CK(X.occl.alloc(cap_rays)); CK(X.ao_weight.alloc(cap_rays));
+    ps.occl = dense_view(X.occl.p);
+    const bool ainst = sc->d.n_instances > 0;  // two-level traversal; the any-hit rays need no instance record of their own
+    if (ainst) { CK(X.hit_inst.alloc(std::max(cap_paths, cap_rays))); ps.hit_inst = X.hit_inst.p; }
+    uint32_t* d_nrays = X.counts.p + 3;
+    TraceIO io;
+    std::memset(&io, 0, sizeof io);
+    io.rays = X.rays.p; io.hit = ps.hit; io.mis_hit = ps.hit; io.occl = ps.occl;
+    io.hit_inst = ps.hit_inst; io.mis_inst = ps.hit_inst; io.instancing = rp.instancing;
+    TraceLauncher tl;
+    CK(tl.init(sc, R.p->flags, sm_count_of(sc->device), R.knobs));
+    for (const BatchInfo& bi : B.batches) {
+        const uint32_t n = bi.n_pixels * bi.n_samples;
+        CK(cudaMemsetAsync(d_nrays, 0, 4, st));
+        launch_raygen(R, sc, sc->d, ps, bi, cam_sobol_p, X, st);
+        TRY(trace_step(R, scr, tl, sc, sc->d, io, X.counts.p, st, true, nullptr));
+        CK(cudaMemsetAsync(d_nrays, 0, 4, st));
+        cudaEvent_t e, f;
+        CK(scr->event(&e)); CK(scr->event(&f));
+        CK(cudaEventRecord(e, st));
+        const uint64_t total = (uint64_t)n * ao_n;
+        k_ao_shade<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(sc->d, rp, ps, bi, ao_n, p->ao_cos_sample ? 1u : 0u, sc->nib.p, n_chunks, sc->vdc.p,
+                                                                 sc->vdci.p, X.rays.p, X.ao_weight.p, d_nrays);
+        CK(cudaEventRecord(f, st));
+        R.sev.push_back(e); R.sev.push_back(f);
+        R.launches++;
+        TRY(trace_step(R, scr, tl, sc, sc->d, io, X.counts.p, st, true, nullptr));
+        k_ao_resolve<<<(n + 255) / 256, 256, 0, st>>>(ps, bi, ao_n, X.ao_weight.p, X.occl.p);
+        R.launches++;
+        launch_resolve(R, sc, scr, ps, bi, X, st);
+    }
+    CK(cudaGetLastError());
+    return end_frame(R);
+}
+
+// The launches of one k_shade step: {specialisation, first class, one past the last class}.  Every single-lobe class the scene has
+// gets its own instantiation (the Lambert one exists for every sampler / light / instancing combination, the others for the Sobol'
+// sampler without instances: what the benchmark configurations run); class 0 ("nothing to shade") and the null-material hits of
+// class 1 ride with the first launch; what is left goes to the general instantiation.  Image lights: one general launch over every class.
+struct ShadeLaunch { int spec; uint32_t lo, hi; };
+static std::vector<ShadeLaunch> shade_plan(const PbrtScene* sc, const PbrtRenderParams* p, int shade_spec, bool halton) {
+    std::vector<ShadeLaunch> plan;
+    if (sc->light_level >= 2) {
+        plan.push_back({0, 1u, (uint32_t)PB_SHADE_CLASSES});
+        return plan;
+    }
+    const bool instanced = sc->d.n_instances > 0;
+    uint32_t mask = sc->class_mask & ~1u, covered = 0;
+    const uint32_t first_general = PB_SPEC_PLASTIC + 1;
+    for (uint32_t c = 1; c < first_general && shade_spec; ++c) {
+        if (!(mask & (1u << c))) continue;
+        const bool have = c == 1 + LOBE_LAMBERT || (shade_spec >= 2 && !halton && !instanced && (c == 1 + LOBE_SPEC_REFL || c == 1 + LOBE_FRESNEL_SPEC || c == 1 + LOBE_OREN_NAYAR ||
+                                                                                           c == 1 + LOBE_MF_REFL || c == 1 + LOBE_FRESNEL_BLEND || c == PB_SPEC_PLASTIC));
+        if (!have) continue;
+        plan.push_back({(int)c, c, c + 1});
+        covered |= 1u << c;
+    }
+    // the classes no specialised launch covers, as maximal runs, for the general instantiation
+    const uint32_t rest = mask & ~covered;
+    for (uint32_t c = 1; c < PB_SHADE_CLASSES;) {
+        if (!(rest & (1u << c))) { ++c; continue; }
+        uint32_t e = c;
+        while (e < PB_SHADE_CLASSES && (rest & (1u << e))) ++e;
+        plan.push_back({0, c, e});
+        c = e;
+    }
+    // when no material has class 1, the null-material hits that k_sort files under class 1 (a shape without a material, or a
+    // moved instance under quirk Q7): folded into the Lambert launch when nothing lies between, else a launch of their own (the
+    // cheapest instantiation: no BSDF is touched).  An otherwise empty plan keeps that launch too: k_shade resets the counters
+    // the next iteration fills.
+    const uint32_t lam = 1 + LOBE_LAMBERT;
+    const bool null_hits = sc->has_null_material || (instanced && p->instancing == PBRT_INSTANCING_REFERENCE);
+    if (!(mask & 2u) && (null_hits || plan.empty())) {
+        bool folded = false;
+        if ((covered & (1u << lam)) && (mask & ((1u << lam) - 4u)) == 0u)
+            for (ShadeLaunch& l : plan) if (l.spec == (int)lam) { l.lo = 1; folded = true; }
+        if (!folded) plan.insert(plan.begin(), ShadeLaunch{shade_spec ? (int)lam : 0, 1u, 2u});
+    }
+    return plan;
+}
+
+// k_shade's instantiation for (light level, sampler, instancing, specialisation).  Image lights (level 2) only have the general one;
+// instanced scenes take the general-light variants (an instanced scene lit by area lights alone is rare enough); the single-lobe
+// specialisations other than Lambert exist for the Sobol' sampler without instances only.
+using ShadeKernel = decltype(&k_shade<0, false, false, 0>);
+template <int SPEC> static ShadeKernel shade_kernel_any(int light_level, bool halton, bool instanced) {
+    if (halton) return instanced ? k_shade<1, true, true, SPEC> : light_level == 0 ? k_shade<0, true, false, SPEC> : k_shade<1, true, false, SPEC>;
+    return instanced ? k_shade<1, false, true, SPEC> : light_level == 0 ? k_shade<0, false, false, SPEC> : k_shade<1, false, false, SPEC>;
+}
+template <int SPEC> static ShadeKernel shade_kernel_sobol(int light_level) { return light_level == 0 ? k_shade<0, false, false, SPEC> : k_shade<1, false, false, SPEC>; }
+static ShadeKernel shade_kernel(int light_level, bool halton, bool instanced, int spec) {
+    if (light_level >= 2) return halton ? (instanced ? k_shade<2, true, true, 0> : k_shade<2, true, false, 0>) : (instanced ? k_shade<2, false, true, 0> : k_shade<2, false, false, 0>);
+    switch (spec) {
+        case 1 + LOBE_LAMBERT: return shade_kernel_any<1 + LOBE_LAMBERT>(light_level, halton, instanced);
+        case 1 + LOBE_SPEC_REFL: return shade_kernel_sobol<1 + LOBE_SPEC_REFL>(light_level);
+        case 1 + LOBE_FRESNEL_SPEC: return shade_kernel_sobol<1 + LOBE_FRESNEL_SPEC>(light_level);
+        case 1 + LOBE_OREN_NAYAR: return shade_kernel_sobol<1 + LOBE_OREN_NAYAR>(light_level);
+        case 1 + LOBE_MF_REFL: return shade_kernel_sobol<1 + LOBE_MF_REFL>(light_level);
+        case 1 + LOBE_FRESNEL_BLEND: return shade_kernel_sobol<1 + LOBE_FRESNEL_BLEND>(light_level);
+        case PB_SPEC_PLASTIC: return shade_kernel_sobol<PB_SPEC_PLASTIC>(light_level);
+        default: return shade_kernel_any<0>(light_level, halton, instanced);
+    }
+}
+
+// The path integrator's light distribution: the spatial grid's geometry (SpatialLightDistribution::new lightdistrib.rs:127-150) and
+// table rows, or the fixed distribution of the power / uniform strategies
+struct LightPlan {
+    bool spatial = false, sparse = false;
+    int nv[3] = {1, 1, 1};
+    size_t nvox = 1, rows = 1;
+    std::vector<float> fixed_f, fixed_cdf;
+    float fixed_int = 0.0f;
+};
+static LightPlan light_plan(const PbrtScene* sc, uint32_t strategy, size_t budget) {
+    LightPlan L;
+    const uint32_t nl = sc->d.n_lights;
+    L.spatial = strategy == PBRT_LIGHTS_SPATIAL && nl > 0;
+    if (L.spatial) {
+        float diag[3] = {sc->d.wb_max[0] - sc->d.wb_min[0], sc->d.wb_max[1] - sc->d.wb_min[1], sc->d.wb_max[2] - sc->d.wb_min[2]};
+        int me = (diag[0] > diag[1] && diag[0] > diag[2]) ? 0 : (diag[1] > diag[2] ? 1 : 2);
+        float bmax = diag[me];
+        for (int i = 0; i < 3; ++i) {
+            L.nv[i] = std::max(1, f2i_sat(roundf(diag[i] / bmax * 64.0f)));
+            L.nvox *= (size_t)L.nv[i];
+        }
+    }
+    // func + contrib + cdf + func_int of one voxel.  Dense tables for every voxel are the fast path (Cornell: 7 MB); with one
+    // light per emissive triangle they would be nvox x n_lights x 12 bytes (10 k emitters: 31 GB per stream context), so above
+    // the budget the tables become rows handed out on first touch (DLightGrid::row) and the render fails, rather than the
+    // allocation, should the paths visit more voxels than fit.
+    const size_t row_bytes = (3 * std::max<size_t>(nl, 1) + 2) * sizeof(float);
+    L.sparse = L.spatial && L.nvox * row_bytes > budget;
+    L.rows = L.sparse ? std::max<size_t>(1, std::min(L.nvox, budget / row_bytes)) : L.nvox;
+    L.fixed_f.assign(nl, 1.0f);
+    if (!L.spatial && nl > 0) {
+        if (strategy == PBRT_LIGHTS_POWER)  // compute_light_power_distribution integrator.rs:574-584, diffuse.rs:85-93
+            for (uint32_t j = 0; j < nl; ++j) {
+                const DLight& l = sc->h_lights[j];
+                Sp pw;
+                const Sp I = mksp(l.L[0], l.L[1], l.L[2]);
+                if (l.kind == PBRT_LIGHT_POINT) pw = I * (4.0f * PB_PI);  // point.rs / spot.rs / distant.rs power()
+                else if (l.kind == PBRT_LIGHT_SPOT) pw = I * 2.0f * PB_PI * (1.0f - 0.5f * (l.cos_falloff_start + l.cos_total_width));
+                else if (l.kind == PBRT_LIGHT_DISTANT) pw = I * PB_PI * sc->d.world_radius * sc->d.world_radius;
+                else if (l.kind == PBRT_LIGHT_INFINITE) pw = sc->h_env_power[j] * sp1(PB_PI * sc->d.world_radius * sc->d.world_radius);  // infinite.rs:349-355
+                else if (l.kind == PBRT_LIGHT_GONIOMETRIC || l.kind == PBRT_LIGHT_PROJECTION) pw = sc->h_env_power[j];
+                else pw = I * (l.two_sided ? 2.0f : 1.0f) * l.area * PB_PI;
+                L.fixed_f[j] = lum(pw);
+            }
+        make_distribution(L.fixed_f, L.fixed_cdf, L.fixed_int);
+    }
+    return L;
+}
+
+struct PathCtx {  // one batch context of the path integrator
+    DPaths ps; DLightGrid grid; TraceIO io;
+    uint32_t *counts, *d_err, *d_nrays, *d_cursor, *d_cls_count;
+    cudaStream_t s;
+    int cur;
+    int iter;
+};
+// Batch context X's buffers for `cap` camera samples, its views and light-grid tables, on its own stream (behind ev_start) when
+// batches overlap
+static int path_context(RenderCall& R, const PbrtScene* sc, BatchCtx& X, PathCtx& V, size_t cap, const LightPlan& lp, bool dual, cudaEvent_t ev_start) {
+    const Knobs& K = R.knobs;
+    const uint32_t nl = sc->d.n_lights;
+    if (dual) {
+        if (!X.stream) CK(cudaStreamCreateWithFlags(&X.stream, cudaStreamNonBlocking));
+        V.s = X.stream;
+        CK(cudaStreamWaitEvent(V.s, ev_start, 0));
+    } else V.s = R.st;
+    if (K.state_aos) { for (int i = 0; i < 3; ++i) CK(X.rec[i].alloc(4 * cap)); CK(X.f4[3].alloc(cap)); }
+    else {
+        for (int i = 0; i < 9; ++i) CK(X.f4[i].alloc(cap));
+        CK(X.occl.alloc(cap)); CK(X.sobol.alloc(cap)); CK(X.dim.alloc(cap));
+    }
+    CK(X.rays.alloc(2 * 3 * cap));  // up to three rays (path, MIS, shadow) per slot and bounce
+    CK(X.pfilm.alloc(cap));
+    if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
+    CK(X.queue[0].alloc(cap)); CK(X.queue[1].alloc(cap)); CK(X.counts.alloc(8 + 2 * PB_SHADE_CLASSES));
+    CK(X.cls_queue.alloc((size_t)PB_SHADE_CLASSES * cap));
+    CK(X.g_state.alloc(lp.nvox)); CK(X.g_func.alloc(lp.rows * std::max<size_t>(nl, 1))); CK(X.g_cdf.alloc(lp.rows * (nl + 1)));
+    CK(X.g_fint.alloc(lp.rows)); CK(X.g_contrib.alloc(lp.rows * std::max<size_t>(nl, 1))); CK(X.g_request.alloc(lp.nvox + 3));
+    if (lp.sparse) CK(X.g_row.alloc(lp.nvox));
+    DPaths& ps = V.ps;
+    if (K.state_aos) {  // three 64-byte records per slot (pb_scene.cuh::DPaths)
+        auto f4 = [](float4* base, int k) { StridedView<float4> v; v.p = base + k; v.stride = 4; return v; };
+        float4 *A = X.rec[0].p, *B = X.rec[1].p, *C = X.rec[2].p;
+        // (L + flags stay a dense array: k_sort reads the flags word of every slot and k_resolve walks L in slot order)
+        ps.L = dense_view(X.f4[3].p); ps.ray_d = f4(A, 1); ps.beta = f4(A, 2);
+        ps.sobol.p = reinterpret_cast<uint2*>(A + 3); ps.sobol.stride = 8;
+        ps.dim.p = reinterpret_cast<uint32_t*>(A + 3) + 2; ps.dim.stride = 16;
+        ps.ld_light = f4(B, 0); ps.mis_d = f4(B, 1); ps.mis_f = f4(B, 2); ps.nee_beta = f4(B, 3);
+        ps.hit = f4(C, 0); ps.mis_hit = f4(C, 1);
+        ps.occl.p = reinterpret_cast<uint32_t*>(C + 2); ps.occl.stride = 16;
+        ps.path_rec = A;
+    } else {
+        ps.path_rec = nullptr;
+        ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
+        ps.ld_light = dense_view(X.f4[4].p); ps.mis_hit = dense_view(X.f4[5].p); ps.mis_d = dense_view(X.f4[6].p); ps.mis_f = dense_view(X.f4[7].p);
+        ps.nee_beta = dense_view(X.f4[8].p);
+        ps.occl = dense_view(X.occl.p); ps.sobol = dense_view(X.sobol.p); ps.dim = dense_view(X.dim.p);
+    }
+    ps.p_film = X.pfilm.p;
+    if (sc->d.n_instances > 0) { CK(X.hit_inst.alloc(cap)); CK(X.mis_inst.alloc(cap)); }
+    ps.hit_inst = X.hit_inst.p; ps.mis_inst = X.mis_inst.p;
+    ps.ray_diff = nullptr; ps.slot_mat = nullptr; ps.slot_frame = nullptr;
+    if (sc->d.n_textures > 0) {
+        CK(X.ray_diff.alloc(3 * cap)); CK(X.slot_mat.alloc(cap)); CK(X.slot_frame.alloc(2 * cap));
+        ps.ray_diff = X.ray_diff.p; ps.slot_mat = X.slot_mat.p; ps.slot_frame = X.slot_frame.p;
+    }
+    DLightGrid& g = V.grid;
+    std::memset(&g, 0, sizeof g);
+    g.n_lights = (int)nl;
+    g.nv[0] = lp.nv[0]; g.nv[1] = lp.nv[1]; g.nv[2] = lp.nv[2];
+    g.state = X.g_state.p; g.func = X.g_func.p; g.cdf = X.g_cdf.p; g.func_int = X.g_fint.p;
+    g.contrib = X.g_contrib.p; g.request = X.g_request.p; g.n_request = X.g_request.p + lp.nvox;
+    g.row = lp.sparse ? X.g_row.p : nullptr;
+    g.max_rows = (uint32_t)lp.rows;
+    CK(cudaMemsetAsync(g.state, 0, lp.nvox * sizeof(int), V.s));
+    CK(cudaMemsetAsync(g.n_request, 0, 3 * sizeof(uint32_t), V.s));
+    if (lp.sparse) CK(cudaMemsetAsync(g.row, 0, lp.nvox * sizeof(int), V.s));
+    if (!lp.spatial && nl > 0) {
+        CK(cudaMemcpyAsync(g.func, lp.fixed_f.data(), nl * 4, cudaMemcpyHostToDevice, V.s));
+        CK(cudaMemcpyAsync(g.cdf, lp.fixed_cdf.data(), (nl + 1) * 4, cudaMemcpyHostToDevice, V.s));
+        CK(cudaMemcpyAsync(g.func_int, &lp.fixed_int, 4, cudaMemcpyHostToDevice, V.s));
+    }
+    V.counts = X.counts.p; V.d_err = X.counts.p + 2; V.d_nrays = X.counts.p + 3; V.d_cursor = X.counts.p + 4; V.d_cls_count = X.counts.p + 8;
+    CK(cudaMemsetAsync(X.counts.p, 0, (8 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
+    std::memset(&V.io, 0, sizeof V.io);
+    V.io.rays = X.rays.p; V.io.hit = ps.hit; V.io.mis_hit = ps.mis_hit; V.io.occl = ps.occl;
+    V.io.hit_inst = ps.hit_inst; V.io.mis_inst = ps.mis_inst; V.io.instancing = R.rp.instancing;
+    V.cur = 0;
+    if (K.ray_sort) { CK(X.ray_keys.alloc(3 * cap)); CK(X.ray_perm.alloc(3 * cap)); CK(X.ray_hist.alloc(PB_RAY_KEYS)); }
+    if (K.ray_prep) CK(X.rays_pre.alloc(2 * 3 * cap));
+    return PBRT_OK;
+}
+
+// ---- PathIntegrator: each batch of camera samples runs trace -> sort -> light grid -> shade iterations, max_depth + 1 of them, or
+// through null surfaces as many as the device reports; up to four batches in flight on as many streams.
+static int render_path(PbrtScene* sc, DeviceScratch* scr, RenderCall& R) {
+    const PbrtRenderParams* p = R.p;
+    const DRender& rp = R.rp;
+    const Knobs& K = R.knobs;
+    const cudaStream_t st = R.st;
+    const bool halton = rp.halton != 0;
+    const bool instanced = sc->d.n_instances > 0;
+    const bool textured = sc->d.n_textures > 0;
+    // paths can walk through surfaces without counting a bounce (Material "none"; in PBRT_INSTANCING_REFERENCE every transformed
+    // instance hit): the number of iterations is not bounded by max_depth, the queue is polled from the host.  The same loop serves a large
+    // "maxdepth" (a legitimate setting: the paths then end by Russian roulette, path.rs:253-262): the fixed-length loop below would queue max_depth + 1
+    // iterations over queues that have long been empty -- and never finish for the u32 maximum.
+    const bool null_paths = sc->has_null_material || (instanced && p->instancing == PBRT_INSTANCING_REFERENCE) || rp.max_depth > 64u;
+    // Camera samples in flight per batch.  2^24 (6 GB of wavefront state per stream context): every batch ends in one or two iterations
+    // that hold a few thousand rays and still last as long as one ray's chain of dependent fetches, so fewer, larger batches spend
+    // less of the frame in those tails (the statue and shares of its frame gain; Cornell and the conference scene are indifferent).
+    // Two contexts of 2^24 take 12 GB, well inside an 80 GB H100.
+    // Scenes with textured materials stay at 2^22: k_texture leaves a 496-byte lobe record per hit (8 GB per context at 2^24) that k_shade
+    // reads back through the class-sorted queue, and k_shade's time per slot grows with that working set.
+    const BatchPlan B = batch_plan(rp.spp, R.share_pixels, 1u << (K.batch_log2 ? K.batch_log2 : (textured ? 22 : 24)));
+    const size_t cap = B.cap;
+    const std::vector<ShadeLaunch> plan = shade_plan(sc, p, K.shade_spec, halton);
+    // Two batches in flight on two streams: k_trace and k_shade leave the SMs idle in different ways, so letting one batch
+    // trace while the other shades fills the SMs better than either alone.  Disabled for the roofline timing pass
+    // (PBRT_RENDER_SINGLE_STREAM: kernel durations must not be inflated by a co-resident kernel), when the queue
+    // has to be polled from the host (null materials), and when there is only one batch.
+    // ... and when an iteration is a single k_shade launch.  On an H100 at 400 W (DESIGN.md section 7) the statue, two launches per
+    // iteration, renders at 1 629-1 637 Mrays/s with two batches in flight against 1 574-1 585 with one; Cornell, one Lambert launch,
+    // cannot be told apart (2 873-2 953 against 2 902-2 969), so it keeps one stream.  PB_STREAMS = 1 keeps one batch in flight,
+    // PB_STREAMS >= 2 forces two.
+    // A textured frame is bound by k_texture's per-hit records (written once, read back by k_shade): a second batch in flight doubles that
+    // working set and loses.
+    const bool dual = !K.single_stream && !(p->flags & PBRT_RENDER_SINGLE_STREAM) && !null_paths && B.batches.size() > 1 && K.streams != 1 &&
+                      ((plan.size() >= 2 && !textured) || K.streams >= 2);
+    const int n_ctx = dual ? (int)std::min<uint64_t>((uint64_t)(K.streams ? K.streams : 2), B.batches.size()) : 1;
+    const int sm_count = sm_count_of(sc->device);
+    const LightPlan lp = light_plan(sc, rp.light_strategy, K.lightgrid_bytes);
+    TRY(upload_filter(R, scr));
+
+    // Sobol' dimensions reachable by this render: 5 camera dims + 8 per shaded bounce
+    const uint32_t dims_needed = (uint32_t)std::min<uint64_t>(1024u, 5 + 8 * ((uint64_t)rp.max_depth + 1));
+    const uint32_t n_chunks = sobol_chunks(rp, rp.spp);
+    // this render's transposed nibble-table slice nibT[(chunk*16+e)*ds + dim], padded by 8 dimensions (pb_sobol.cuh)
+    const uint32_t sobol_ds = (dims_needed + 8u) | 1u;
+    {
+        std::vector<uint32_t>& T = scr->h_nibT;
+        T.assign((size_t)n_chunks * 16 * sobol_ds, 0u);
+        for (uint32_t c = 0; c < n_chunks; ++c)
+            for (uint32_t e = 0; e < 16; ++e)
+                for (uint32_t d = 0; d < dims_needed; ++d) T[((size_t)c * 16 + e) * sobol_ds + d] = sc->h_nib[((size_t)d * PB_SOBOL_CHUNKS + c) * 16 + e];
+        CK(scr->nibT.alloc(T.size()));
+        CK(cudaMemcpyAsync(scr->nibT.p, T.data(), T.size() * 4, cudaMemcpyHostToDevice, st));
+    }
+    const bool stage_sobol = (size_t)sobol_ds * n_chunks * 64 <= PB_SMEM_SOBOL_BYTES;
+    const uint32_t sobol_cfg = sobol_ds | (stage_sobol ? 0x80000000u : 0u);
+    const size_t shade_smem = halton || !stage_sobol ? 0 : (size_t)sobol_ds * n_chunks * 64;
+    const uint4* cam_sobol_p = nullptr;  // (on the caller's stream, ahead of ev_start: every context's k_raygen reads it)
+    TRY(camera_sobol(R, scr, sc, n_chunks, &cam_sobol_p));
+    TraceLauncher tl;
+    CK(tl.init(sc, p->flags, sm_count, K));
+    // With batches in flight on several streams each stream's persistent trace grid takes 3/(2*n_ctx) of the resident CTAs -- 6 of 8
+    // per SM with two streams -- not an even 1/n_ctx share: a batch that traces while its partner shades or sorts cannot grow into the
+    // idle half, and an even share left it at half occupancy then.  When both trace at once, the CTAs that do not fit wait for free
+    // slots and take what is left of their queue.  On an H100 the statue rendered about 3 % faster than with 4 of 8 (DESIGN.md section 7).
+    tl.grid = sm_count * std::max(1, n_ctx > 1 ? std::max(tl.blocks_per_sm, 1) * 3 / (2 * n_ctx) : std::max(tl.blocks_per_sm, 1));
+    const int shade_grid = sm_count * (8 / n_ctx);
+    int shade_grid_spec = shade_grid;  // the Lambert launch's
+    if (K.shade_spec) {
+        int bps = 4;
+        // (an image-lit scene has no Lambert launch: it asks for the level-1 kernel and never uses the answer)
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, shade_kernel(std::min(sc->light_level, 1), halton, instanced, 1 + LOBE_LAMBERT), PB_SHADE_THREADS, shade_smem));
+        shade_grid_spec = sm_count * std::max(1, std::max(bps, 1) / n_ctx);
+    }
+    PathCtx live[4];
+    cudaEvent_t ev_start;
+    CK(scr->event(&ev_start));
+    CK(cudaEventRecord(ev_start, st));
+    for (int c = 0; c < n_ctx; ++c) TRY(path_context(R, sc, scr->ctx[c], live[c], cap, lp, dual, ev_start));
+
+    // ---- one iteration (trace -> sort -> light grid -> shade) of the batch living in context c ----
+    // `stagger` (first iteration of a batch pair): context 1 starts tracing only when context 0 has finished its
+    // first trace, so that from then on one batch traces while the other shades
+    cudaEvent_t ev_stagger[4];
+    for (int i = 0; i < 4; ++i) CK(scr->event(&ev_stagger[i]));
+    auto enqueue_iteration = [&](int c, bool stagger) -> int {
+        BatchCtx& X = scr->ctx[c];
+        PathCtx& V = live[c];
+        const cudaStream_t s = V.s;
+        const int cur = V.cur;
+        uint32_t* c_in = V.counts + cur;
+        uint32_t* c_out = V.counts + (cur ^ 1);
+        uint32_t* cls_now = V.d_cls_count + PB_SHADE_CLASSES * (V.iter & 1);        // filled by this iteration's k_sort
+        uint32_t* cls_next = V.d_cls_count + PB_SHADE_CLASSES * ((V.iter + 1) & 1);  // cleared by this iteration's k_shade
+        if (stagger && c >= 1) CK(cudaStreamWaitEvent(s, ev_stagger[c - 1], 0));
+        // camera rays arrive in pixel order (coherent as they are); every later queue is bucketed by direction / origin
+        V.io.perm = nullptr;
+        if (K.ray_sort && V.iter > 0) {
+            CK(cudaMemsetAsync(X.ray_hist.p, 0, PB_RAY_KEYS * sizeof(uint32_t), s));
+            k_ray_hist<<<sm_count * 4, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p);
+            k_ray_scan<<<1, 1024, 0, s>>>(X.ray_hist.p);
+            if (K.ray_sort == 2) k_ray_scatter2<<<sm_count * 8, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p, X.ray_perm.p);
+            else k_ray_scatter<<<sm_count * 8, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p, X.ray_perm.p);
+            R.launches += 3;
+            V.io.perm = X.ray_perm.p;
+        }
+        V.iter++;
+        TRY(trace_step(R, scr, tl, sc, sc->d, V.io, V.counts, s, false, K.ray_prep ? X.rays_pre.p : nullptr));
+        if (stagger) CK(cudaEventRecord(ev_stagger[c], s));
+        k_sort<<<sm_count * 8, 256, 0, s>>>(sc->d, V.ps, V.grid, lp.spatial ? 1u : 0u, rp.instancing, X.queue[cur].p, c_in, X.cls_queue.p, (uint32_t)cap, cls_now, c_out,
+                                            V.d_nrays);
+        R.launches++;
+        if (textured) {  // V.iter == 1: the rays just traced are the camera rays, the only ones with differentials (none from an environment camera)
+            k_texture<<<sm_count * 8, 128, 0, s>>>(sc->d, rp, V.ps, X.queue[cur].p, c_in, V.iter == 1 && sc->cam_kind != PBRT_CAMERA_ENVIRONMENT ? 1u : 0u);
+            R.launches++;
+        }
+        if (lp.spatial) {
+            if (sc->light_level >= 2) k_lightgrid_contrib<2><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
+            else k_lightgrid_contrib<1><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
+            k_lightgrid_build<<<sm_count, 128, 0, s>>>(V.grid);
+            R.launches += 2;
+        }
+        cudaEvent_t e, f;
+        CK(scr->event(&e)); CK(scr->event(&f));
+        CK(cudaEventRecord(e, s));
+        for (const ShadeLaunch& sl : plan) {
+            const ShadeKernel shade = shade_kernel(sc->light_level, halton, instanced, sl.spec);
+            const int grid = sl.spec == 1 + LOBE_LAMBERT ? shade_grid_spec : shade_grid;
+            shade<<<grid, PB_SHADE_THREADS, shade_smem, s>>>(sc->d, rp, V.ps, V.grid, scr->nibT.p, sobol_cfg, n_chunks, X.cls_queue.p, (uint32_t)cap, cls_now,
+                                                            X.queue[cur ^ 1].p, c_out, X.rays.p, V.d_nrays, sc->counters.p, V.d_err,
+                                                            K.ray_sort ? X.ray_keys.p : nullptr, K.ray_key_mask, V.d_cursor,
+                                                            lp.spatial ? V.grid.n_request : nullptr, cls_next, sl.lo, sl.hi);
+            R.launches++;
+        }
+        CK(cudaEventRecord(f, s));
+        R.sev.push_back(e); R.sev.push_back(f);
+        V.cur ^= 1;
+        return PBRT_OK;
+    };
+    // null_paths: the number of iterations is only known on the device (one batch context); the queue length is polled late, and
+    // the iteration queued past the end runs over empty queues, like the tail iterations of the fixed-length loop
+    LatePoll poll;
+    if (null_paths) TRY(poll.init(scr, K.poll_lag));
+
+    R.since("setup done");
+    // batches are dealt to the contexts round robin; the host interleaves the two streams' launches at
+    // iteration granularity so both always have work queued
+    for (size_t b0 = 0; b0 < B.batches.size(); b0 += (size_t)n_ctx) {
+        const int nb = (int)std::min<size_t>((size_t)n_ctx, B.batches.size() - b0);
+        for (int c = 0; c < nb; ++c) {
+            PathCtx& V = live[c];
+            V.cur = 0;
+            V.iter = 0;
+            // ray count, ray cursor, both sets of class counts (and the voxel requests): from here on the kernels reset them for each other
+            CK(cudaMemsetAsync(V.d_nrays, 0, (5 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
+            if (lp.spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
+            launch_raygen(R, sc, sc->d, V.ps, B.batches[b0 + c], cam_sobol_p, scr->ctx[c], V.s);
+        }
+        for (uint32_t it = 0; null_paths || it < rp.max_depth + 1; ++it) {
+            for (int c = 0; c < nb; ++c) TRY(enqueue_iteration(c, dual && nb >= 2 && it == 0));
+            bool done = false;
+            if (null_paths) TRY(poll.poll(it, live[0].counts + live[0].cur, live[0].s, &done));
+            if (done) break;
+        }
+        for (int c = 0; c < nb; ++c) launch_resolve(R, sc, scr, live[c].ps, B.batches[b0 + c], scr->ctx[c], live[c].s);
+    }
+    CK(cudaGetLastError());
+    R.since("all batches enqueued");
+    // join the side streams back into the caller's stream
+    if (dual)
+        for (int c = 0; c < n_ctx; ++c) {
+            cudaEvent_t done;
+            CK(scr->event(&done));
+            CK(cudaEventRecord(done, live[c].s));
+            CK(cudaStreamWaitEvent(st, done, 0));
+        }
+    uint32_t errs[4] = {0, 0, 0, 0}, grid_full[4] = {0, 0, 0, 0};
+    for (int c = 0; c < n_ctx; ++c) CK(cudaMemcpyAsync(&errs[c], live[c].d_err, 4, cudaMemcpyDeviceToHost, st));
+    if (lp.sparse)
+        for (int c = 0; c < n_ctx; ++c) CK(cudaMemcpyAsync(&grid_full[c], live[c].grid.n_request + 2, 4, cudaMemcpyDeviceToHost, st));
+    TRY(end_frame(R));
+    R.since("final sync");
+    if (grid_full[0] | grid_full[1] | grid_full[2] | grid_full[3])
+        return fail(PBRT_E_UNSUPPORTED, "spatial light distribution: the paths touch more voxels than the table budget holds (PB_LIGHTGRID_BYTES, "
+                                        "default 4 GiB per stream context); render with the power or uniform light strategy");
+    return errs[0] | errs[1] | errs[2] | errs[3] ? fail_dims(rp) : PBRT_OK;
+}
+
+static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& share, float* d_film, float* d_samples, cudaStream_t st,
+                       PbrtStats* stats) {
+    const bool tiled = share.n_parts > 0;
+    const int32_t* rect_in = tiled ? (p ? p->sample_bounds : nullptr) : share.rect;
+    if (!sc || !p || !rect_in) return fail(PBRT_E_INVALID, "null argument");
+    if (tiled && share.part >= share.n_parts) return fail(PBRT_E_INVALID, "tile share out of range");
+    if (tiled && d_samples) return fail(PBRT_E_INVALID, "per-sample output needs a pixel rectangle");
+    RenderCall R;
+    R.p = p; R.d_film = d_film; R.d_samples = d_samples; R.st = st;
+    R.knobs = knobs();
+    R.device = sc->device;
+    R.t_enter = std::chrono::steady_clock::now();
+    CK(cudaSetDevice(sc->device));
+    std::vector<uint32_t> h_tiles;
+    TRY(render_setup(sc, p, share, rect_in, R, h_tiles));
+    DRender& rp = R.rp;
 
     DeviceScratch* scr = scratch_for(sc->device);
     if (!scr) return fail(PBRT_E_INVALID, "device ordinal out of range");
     std::lock_guard<std::mutex> scratch_lock(scr->mu);
-    if (tiled && !h_tiles.empty()) {
+    if (!h_tiles.empty()) {
         CK(scr->tiles.alloc(h_tiles.size()));
         CK(cudaMemcpyAsync(scr->tiles.p, h_tiles.data(), h_tiles.size() * 4, cudaMemcpyHostToDevice, st));  // (h_tiles outlives the render: synchronised below)
         rp.tiles = scr->tiles.p;
         rp.n_tiles = (uint32_t)h_tiles.size();
     }
-    if (halton) {  // HaltonSampler::new (halton.rs:84-112)
-        rp.halton = 1u;
-        rp.h_center = p->sample_at_pixel_center ? 1u : 0u;
-        const int res[2] = {rp.sb[2] - rp.sb[0], rp.sb[3] - rp.sb[1]};
-        for (int i = 0; i < 2; ++i) {
-            const int base = i == 0 ? 2 : 3;
-            int scale = 1, e = 0;
-            while (scale < std::min(res[i], 128)) { scale *= base; e += 1; }
-            rp.h_scale[i] = (uint32_t)scale;
-            rp.h_exp[i] = (uint32_t)e;
-        }
-        rp.h_stride = rp.h_scale[0] * rp.h_scale[1];
-        rp.h_mult[0] = (uint32_t)halton_mult_inverse(rp.h_scale[1], rp.h_scale[0]);
-        rp.h_mult[1] = (uint32_t)halton_mult_inverse(rp.h_scale[0], rp.h_scale[1]);
-        if ((uint64_t)rp.spp * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 (spp * 128 * 243) are outside the GPU path");
-        const HaltonTables& T = halton_tables();
-        if (!scr->h_dims.p) {
-            CK(scr->h_dims.upload(T.dims));
-            CK(scr->h_perm.upload(T.perms));
-        }
-        rp.h_dims = scr->h_dims.p;
-        rp.h_perm = scr->h_perm.p;
-    }
-    cudaEvent_t ev0, ev1;
+    if (p->sampler == PBRT_SAMPLER_HALTON) TRY(halton_setup(scr, p, rp));
+    cudaEvent_t ev0;
     scr->ev_used = 0;
-    CK(scr->event(&ev0)); CK(scr->event(&ev1));
-    std::vector<cudaEvent_t> tev, sev;  // per-launch event pairs for the trace / shade kernels
+    CK(scr->event(&ev0)); CK(scr->event(&R.ev1));
     CK(sc->counters.alloc(1));
     CK(cudaMemsetAsync(sc->counters.p, 0, sizeof(DCounters), st));
     CK(cudaEventRecord(ev0, st));
-    uint32_t launches = 0, trace_launches = 0;
 
     if (p->integrator > PBRT_INTEGRATOR_WHITTED) return fail(PBRT_E_UNSUPPORTED, "integrator outside the GPU path");
-    if (sc->d.n_textures || p->integrator >= PBRT_INTEGRATOR_DIRECT) {
-        // k_texture and k_direct_step keep a DMaterial (and a texture-graph stack) in local memory: stack frames of ~1.5 KB, above the
-        // default per-thread stack limit of 1 KB.  Raise it once per device (a no-op if the driver sizes known frames by itself).
-        size_t cur = 0;
-        CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
-        if (cur < 4096) CK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
-    }
+    if (sc->d.n_textures || p->integrator >= PBRT_INTEGRATOR_DIRECT) TRY(raise_stack_limit());
     const bool direct = p->integrator == PBRT_INTEGRATOR_DIRECT || p->integrator == PBRT_INTEGRATOR_WHITTED;
     if (direct && p->direct_strategy > PBRT_DIRECT_SAMPLE_ONE) return fail(PBRT_E_INVALID, "unknown direct-lighting strategy");
     if (p->instancing > PBRT_INSTANCING_FIXED) return fail(PBRT_E_INVALID, "unknown instancing mode");
     rp.instancing = p->instancing;
-    // paths can walk through surfaces without counting a bounce (Material "none"; in PBRT_INSTANCING_REFERENCE every transformed
-    // instance hit): the number of iterations is not bounded by max_depth, the queue is polled from the host.  The same loop serves a large
-    // "maxdepth" (a legitimate setting: the paths then end by Russian roulette, path.rs:253-262): the fixed-length loop below would queue max_depth + 1
-    // iterations over queues that have long been empty -- and never finish for the u32 maximum.
-    const bool null_paths = sc->has_null_material || (sc->d.n_instances > 0 && p->instancing == PBRT_INSTANCING_REFERENCE) || rp.max_depth > 64u;
-    const bool ao = p->integrator == PBRT_INTEGRATOR_AO;
-    if (direct && share_pixels > 0) {
-        // ---- DirectLightingIntegrator / WhittedIntegrator (pb_direct.cuh): raygen -> trace -> { k_direct_step -> k_direct_nee -> trace }
-        // until every camera sample's tree is walked -> k_resolve, one batch at a time on the caller's stream.
-        const bool whitted = p->integrator == PBRT_INTEGRATOR_WHITTED;
-        const bool sample_all = !whitted && p->direct_strategy == PBRT_DIRECT_SAMPLE_ALL;
-        const uint32_t nl = sc->d.n_lights;
-        if (rp.max_depth > PB_DIRECT_MAX_DEPTH) return fail(PBRT_E_UNSUPPORTED, "direct / whitted maxdepth beyond 8 is outside the GPU path");
-        std::vector<uint32_t> nee_light, nee_k, light_n(nl), light_q0(nl);
-        uint32_t max_n = 1;
-        for (uint32_t j = 0; j < nl; ++j) {
-            light_n[j] = sample_all ? std::max(1u, sc->h_lights[j].n_samples) : 1u;
-            light_q0[j] = (uint32_t)nee_light.size();
-            max_n = std::max(max_n, light_n[j]);
-            if (sample_all || whitted) for (uint32_t k = 0; k < light_n[j]; ++k) { nee_light.push_back(j); nee_k.push_back(k); }
-        }
-        if (!sample_all && !whitted) { nee_light.assign(1, 0u); nee_k.assign(1, 0u); }
-        if (nee_light.empty()) { nee_light.assign(1, 0u); nee_k.assign(1, 0u); }  // no lights: k_direct_nee never has work
-        const uint32_t n_nee = (uint32_t)nee_light.size();
-        if (n_nee > 4096) return fail(PBRT_E_UNSUPPORTED, "more than 4096 light samples per vertex are outside the GPU path");
-        DDirect dd;
-        std::memset(&dd, 0, sizeof dd);
-        dd.max_depth = rp.max_depth; dd.n_nee = n_nee; dd.whitted = whitted ? 1u : 0u; dd.sample_all = sample_all ? 1u : 0u;
-        dd.n_arrays = sample_all ? 2u * nl * rp.max_depth : 0u;
-        dd.array_end = 5u + 2u * dd.n_arrays;
-        const uint64_t array_samples = (uint64_t)rp.spp * max_n;  // pixel sample numbers the 2D arrays reach
-        uint32_t log2_arr = 0;
-        while ((1ull << log2_arr) < array_samples) log2_arr++;
-        if (halton) {
-            if (array_samples * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 are outside the GPU path");
-        } else if (2u * rp.log2_res + log2_arr > 52u) return fail(PBRT_E_UNSUPPORTED, "Sobol' index beyond 52 bits");
-        dd.n_chunks = std::max<uint32_t>(1u, (2u * rp.log2_res + log2_arr + 3u) / 4u);
-        const bool count_work = (p->flags & PBRT_RENDER_COUNT_WORK) != 0;
-        const uint64_t total_pixels = share_pixels;
-        // light samples in flight per batch (PB_SIBLING_BATCH_LOG2: a test hook that forces many small batches)
-        const size_t CAP = (size_t)1 << (getenv("PB_SIBLING_BATCH_LOG2") ? std::min(24, std::max(4, atoi(getenv("PB_SIBLING_BATCH_LOG2")))) : 21);
-        const uint32_t paths_cap = (uint32_t)std::max<size_t>(1, std::min<size_t>((size_t)1 << 20, CAP / n_nee));
-        const uint32_t samples_per_batch = std::min<uint32_t>(rp.spp, paths_cap);
-        const uint32_t pixels_per_batch = (uint32_t)std::min<uint64_t>(std::max<uint32_t>(1u, paths_cap / samples_per_batch), total_pixels);
-        const size_t cap = (size_t)samples_per_batch * pixels_per_batch, cap_nee = cap * n_nee, depth_n = std::max(1u, rp.max_depth);
-        dd.cap = cap;
-        CK(scr->filter_table.alloc(256));
-        CK(cudaMemcpyAsync(scr->filter_table.p, p->filter_table, 256 * 4, cudaMemcpyHostToDevice, st));
-        BatchCtx& X = scr->ctx[0];
-        for (int i = 0; i < 4; ++i) CK(X.f4[i].alloc(cap));
-        CK(X.rays.alloc(2 * (cap + 2 * cap_nee)));
-        CK(X.sobol.alloc(cap)); CK(X.dim.alloc(cap)); CK(X.pfilm.alloc(cap));
-        if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
-        CK(X.queue[0].alloc(cap)); CK(X.counts.alloc(8 + PB_SHADE_CLASSES));
-        DirectBufs& D = scr->direct;
-        const bool dinst = sc->d.n_instances > 0;
-        const bool dtex = sc->d.n_textures > 0;
-        CK(D.u32.alloc(6 * cap + 2 * cap_nee + 2 * (size_t)n_nee + 2 * (size_t)std::max(1u, nl) + (dinst ? cap + cap_nee + depth_n * cap : 0) +
-                       (dtex ? cap + depth_n * cap : 0)));
-        CK(D.f4.alloc(4 * depth_n * cap + 4 * cap_nee + (dtex ? 3 * cap + 3 * depth_n * cap : 0)));
-        uint32_t* u = D.u32.p;
-        dd.state = u; u += cap; dd.depth = reinterpret_cast<int*>(u); u += cap; dd.arr_off = u; u += cap;
-        dd.nee_depth = reinterpret_cast<int*>(u); u += cap; dd.nee_dim = u; u += cap; dd.nee_arr = u; u += cap;
-        // (fresh shares the queue buffer, which this integrator does not use otherwise)
-        dd.fresh = X.queue[0].p;
-        dd.nee_flags = u; u += cap_nee; dd.nee_occl = u; u += cap_nee;
-        uint32_t* t_light = u; u += n_nee; uint32_t* t_k = u; u += n_nee; uint32_t* t_n = u; u += std::max(1u, nl); uint32_t* t_q0 = u; u += std::max(1u, nl);
-        uint32_t *d_hit_inst = nullptr, *d_mis_inst = nullptr;
-        if (dinst) { d_hit_inst = u; u += cap; d_mis_inst = u; u += cap_nee; dd.node_inst = u; u += depth_n * cap; }
-        if (dtex) { dd.cur_has_diff = u; u += cap; dd.node_has_diff = u; u += depth_n * cap; }
-        CK(cudaMemcpyAsync(t_light, nee_light.data(), (size_t)n_nee * 4, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(t_k, nee_k.data(), (size_t)n_nee * 4, cudaMemcpyHostToDevice, st));
-        if (nl) {
-            CK(cudaMemcpyAsync(t_n, light_n.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(t_q0, light_q0.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st));
-        }
-        dd.nee_light = t_light; dd.nee_k = t_k; dd.light_n = t_n; dd.light_q0 = t_q0;
-        float4* f = D.f4.p;
-        dd.node_L = f; f += depth_n * cap; dd.node_mul = f; f += depth_n * cap; dd.node_hit = f; f += depth_n * cap; dd.node_rd = f; f += depth_n * cap;
-        dd.nee_a = f; f += cap_nee; dd.nee_mf = f; f += cap_nee; dd.nee_md = f; f += cap_nee; dd.nee_mis_hit = f; f += cap_nee;
-        if (dtex) { dd.cur_diff = f; f += 3 * cap; dd.node_diff = f; f += 3 * depth_n * cap; }
-        CK(cudaStreamSynchronize(st));  // the tables above come from host vectors that go out of scope with this block's iterations
-        DPaths ps;
-        std::memset(&ps, 0, sizeof ps);
-        ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
-        ps.sobol = dense_view(X.sobol.p); ps.dim = dense_view(X.dim.p); ps.p_film = X.pfilm.p;
-        ps.hit_inst = d_hit_inst; ps.mis_inst = d_mis_inst;
-        if (dtex) {
-            CK(X.ray_diff.alloc(3 * cap)); CK(X.slot_mat.alloc(cap)); CK(X.slot_frame.alloc(2 * cap));
-            ps.ray_diff = X.ray_diff.p; ps.slot_mat = X.slot_mat.p; ps.slot_frame = X.slot_frame.p;
-        }
-        uint32_t* d_count = X.counts.p;
-        uint32_t* d_active2 = X.counts.p + 5;  // two words: iteration i counts into word i & 1, iteration i + 1 reads it
-        uint32_t* d_err = X.counts.p + 2;
-        uint32_t* d_nrays = X.counts.p + 3;
-        uint32_t* d_cursor = X.counts.p + 4;
-        CK(cudaMemsetAsync(d_err, 0, 4, st));
-        TraceIO io;
-        std::memset(&io, 0, sizeof io);
-        io.rays = X.rays.p; io.hit = ps.hit; io.mis_hit = dense_view(dd.nee_mis_hit); io.occl = dense_view(dd.nee_occl);
-        io.hit_inst = d_hit_inst; io.mis_inst = d_mis_inst; io.instancing = rp.instancing;
-        DScene dsc = sc->d;
-        dsc.materials = sc->materials_single.p;  // allow_multiple_lobes = false
-        const int sm_count = sm_count_of(sc->device);
-        TraceLauncher tl;
-        CK(tl.init(sc, count_work, sm_count));
-        auto trace = [&]() -> int {
-            CK(cudaMemsetAsync(d_cursor, 0, 4, st));
-            cudaEvent_t a, b;
-            CK(scr->event(&a)); CK(scr->event(&b));
-            CK(cudaEventRecord(a, st));
-            tl.launch(dsc, io, d_nrays, d_cursor, sc->counters.p, st);
-            CK(cudaEventRecord(b, st));
-            tev.push_back(a); tev.push_back(b);
-            launches++; trace_launches++;
-            return PBRT_OK;
-        };
-        uint32_t log2_spp = 0;
-        while ((1u << log2_spp) < rp.spp) log2_spp++;
-        const uint32_t raygen_chunks = std::max<uint32_t>(1u, (std::min<uint32_t>(52u, 2u * rp.log2_res + log2_spp) + 3u) / 4u);
-        const uint4* cam_sobol_p = nullptr;
-        CK(camera_sobol(scr, sc, rp, std::max(raygen_chunks, dd.n_chunks), st, &cam_sobol_p));
-        launches += halton ? 0 : 1;
-        uint32_t* h_poll = nullptr;
-        cudaEvent_t poll_ev[2];
-        CK(scr->poll_words(&h_poll));
-        CK(scr->event(&poll_ev[0])); CK(scr->event(&poll_ev[1]));
-        for (uint32_t s0 = 0; s0 < rp.spp; s0 += samples_per_batch)
-            for (uint64_t pix0 = 0; pix0 < total_pixels; pix0 += pixels_per_batch) {
-                BatchInfo bi;
-                bi.first_pixel = (uint32_t)pix0;
-                bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
-                bi.first_sample = s0;
-                bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
-                bi.n_samples_magic = magic_of(bi.n_samples);
-                const uint32_t n = bi.n_pixels * bi.n_samples;
-                CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                const auto raygen = raygen_kernel(sc);
-                raygen<<<(n + 255) / 256, 256, 0, st>>>(dsc, rp, ps, bi, cam_sobol_p, X.queue[0].p, d_count, X.rays.p, d_nrays, sc->counters.p, sc->cam_mo,
-                                                        sc->env_res, lens_arg(sc, X));
-                launches++;
-                // the recursion's length is decided on the device (the active word = camera samples that still need an iteration).  The
-                // host reads that word poll_lag() iterations late (see there: 0 by default, measured): with a lag of 1 iteration i + 1 is
-                // already queued when i's count arrives, and the iteration queued past the end sees the previous count at 0 and returns.
-                const uint32_t lag = poll_lag();
-                for (uint32_t iter = 0;; ++iter) {
-                    int rc = trace();
-                    if (rc != PBRT_OK) return rc;
-                    uint32_t* d_active = d_active2 + (iter & 1u);
-                    const uint32_t* d_prev = iter ? d_active2 + ((iter - 1u) & 1u) : nullptr;
-                    CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                    CK(cudaMemsetAsync(d_active, 0, 4, st));
-                    cudaEvent_t e, g;
-                    CK(scr->event(&e)); CK(scr->event(&g));
-                    CK(cudaEventRecord(e, st));
-                    const bool env_start = iter == 0 && sc->cam_kind == PBRT_CAMERA_ENVIRONMENT;  // camera rays without a differential
-                    if (env_start) {
-                        k_direct_start_nodiff<<<(n + 127) / 128, 128, 0, st>>>(dsc, ps, dd, bi);
-                        launches++;
-                    }
-                    k_direct_step<<<(n + 127) / 128, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, iter == 0 && !env_start ? 1u : 0u, X.rays.p, d_nrays, d_active, d_err, d_prev);
-                    const uint64_t total = (uint64_t)n * n_nee;
-                    const unsigned nee_grid = (unsigned)((total + 127) / 128);
-                    if (sc->light_level >= 2) k_direct_nee<2><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
-                    else k_direct_nee<1><<<nee_grid, 128, 0, st>>>(dsc, rp, ps, dd, bi, sc->nib.p, sc->vdc.p, sc->vdci.p, X.rays.p, d_nrays, sc->counters.p, d_err, d_prev);
-                    CK(cudaEventRecord(g, st));
-                    sev.push_back(e); sev.push_back(g);
-                    launches += 2;
-                    CK(cudaMemcpyAsync(&h_poll[iter & 1u], d_active, 4, cudaMemcpyDeviceToHost, st));
-                    CK(cudaEventRecord(poll_ev[iter & 1u], st));
-                    if (iter >= lag) {
-                        CK(cudaEventSynchronize(poll_ev[(iter - lag) & 1u]));
-                        if (h_poll[(iter - lag) & 1u] == 0u) break;
-                    }
-                    if (iter > 100000u) return fail(PBRT_E_CUDA, "direct integrator did not terminate");
-                }
-                const auto resolve = resolve_kernel(sc);
-                resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples, X.cam_weight.p);
-                launches++;
-            }
-        CK(cudaGetLastError());
-        uint32_t h_err = 0;
-        CK(cudaMemcpyAsync(&h_err, d_err, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaEventRecord(ev1, st));
-        CK(cudaStreamSynchronize(st));
-        if (h_err) return fail(PBRT_E_UNSUPPORTED, halton ? "HaltonSampler can only sample 1000 dimensions (halton.rs:256-262)"
-                                                          : "SobolSampler can only sample up to 1024 dimensions (sobol.rs:119-124)");
-    } else if (ao && share_pixels > 0) {
-        // ---- AOIntegrator (integrators/ao.rs): raygen -> trace -> k_ao_shade (ao_n any-hit rays per camera sample) -> trace ->
-        // k_ao_resolve -> k_resolve, one batch at a time on the caller's stream.
-        const uint32_t ao_n = p->ao_samples;
-        if (ao_n == 0 || ao_n > 4096) return fail(PBRT_E_INVALID, "ao nsamples out of range (1..4096)");
-        const uint64_t array_samples = (uint64_t)rp.spp * ao_n;  // pixel sample numbers the 2D array reaches
-        uint32_t log2_arr = 0;
-        while ((1ull << log2_arr) < array_samples) log2_arr++;
-        if (halton) {
-            if (array_samples * rp.h_stride >= (1ull << 32)) return fail(PBRT_E_UNSUPPORTED, "Halton sample indices beyond 2^32 are outside the GPU path");
-        } else if (2u * rp.log2_res + log2_arr > 52u) return fail(PBRT_E_UNSUPPORTED, "Sobol' index beyond 52 bits");
-        const uint32_t n_chunks = std::max<uint32_t>(1u, (2u * rp.log2_res + log2_arr + 3u) / 4u);
-        const uint4* cam_sobol_p = nullptr;
-        CK(camera_sobol(scr, sc, rp, n_chunks, st, &cam_sobol_p));
-        launches += halton ? 0 : 1;
-        const bool count_work = (p->flags & PBRT_RENDER_COUNT_WORK) != 0;
-        const uint64_t total_pixels = share_pixels;
-        const size_t CAP = (size_t)1 << (getenv("PB_SIBLING_BATCH_LOG2") ? std::min(24, std::max(4, atoi(getenv("PB_SIBLING_BATCH_LOG2")))) : 22);  // any-hit rays in flight per batch
-        const uint32_t paths_cap = (uint32_t)std::max<size_t>(1, CAP / ao_n);
-        const uint32_t samples_per_batch = std::min<uint32_t>(rp.spp, paths_cap);
-        const uint32_t pixels_per_batch = (uint32_t)std::min<uint64_t>(std::max<uint32_t>(1u, paths_cap / samples_per_batch), total_pixels);
-        const size_t cap_paths = (size_t)samples_per_batch * pixels_per_batch, cap_rays = cap_paths * ao_n;
-        CK(scr->filter_table.alloc(256));
-        CK(cudaMemcpyAsync(scr->filter_table.p, p->filter_table, 256 * 4, cudaMemcpyHostToDevice, st));
-        BatchCtx& X = scr->ctx[0];
-        for (int i = 0; i < 4; ++i) CK(X.f4[i].alloc(cap_paths));
-        CK(X.rays.alloc(2 * std::max(cap_paths, cap_rays)));
-        CK(X.occl.alloc(cap_rays)); CK(X.ao_weight.alloc(cap_rays));
-        CK(X.sobol.alloc(cap_paths)); CK(X.dim.alloc(cap_paths)); CK(X.pfilm.alloc(cap_paths));
-        if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap_paths));
-        CK(X.queue[0].alloc(cap_paths)); CK(X.counts.alloc(8 + PB_SHADE_CLASSES));
-        DPaths ps;
-        std::memset(&ps, 0, sizeof ps);
-        ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
-        ps.occl = dense_view(X.occl.p); ps.sobol = dense_view(X.sobol.p); ps.dim = dense_view(X.dim.p); ps.p_film = X.pfilm.p;
-        const bool ainst = sc->d.n_instances > 0;  // two-level traversal; the any-hit rays need no instance record of their own
-        if (ainst) { CK(X.hit_inst.alloc(std::max(cap_paths, cap_rays))); ps.hit_inst = X.hit_inst.p; }
-        uint32_t* d_count = X.counts.p;
-        uint32_t* d_nrays = X.counts.p + 3;
-        uint32_t* d_cursor = X.counts.p + 4;
-        TraceIO io;
-        std::memset(&io, 0, sizeof io);
-        io.rays = X.rays.p; io.hit = ps.hit; io.mis_hit = ps.hit; io.occl = ps.occl;
-        io.hit_inst = ps.hit_inst; io.mis_inst = ps.hit_inst; io.instancing = rp.instancing;
-        const int sm_count = sm_count_of(sc->device);
-        TraceLauncher tl;
-        CK(tl.init(sc, count_work, sm_count));
-        auto trace = [&]() -> int {
-            CK(cudaMemsetAsync(d_cursor, 0, 4, st));
-            cudaEvent_t a, b;
-            CK(scr->event(&a)); CK(scr->event(&b));
-            CK(cudaEventRecord(a, st));
-            tl.launch(sc->d, io, d_nrays, d_cursor, sc->counters.p, st);
-            CK(cudaEventRecord(b, st));
-            tev.push_back(a); tev.push_back(b);
-            launches++; trace_launches++;
-            return PBRT_OK;
-        };
-        for (uint32_t s0 = 0; s0 < rp.spp; s0 += samples_per_batch)
-            for (uint64_t pix0 = 0; pix0 < total_pixels; pix0 += pixels_per_batch) {
-                BatchInfo bi;
-                bi.first_pixel = (uint32_t)pix0;
-                bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
-                bi.first_sample = s0;
-                bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
-                bi.n_samples_magic = magic_of(bi.n_samples);
-                const uint32_t n = bi.n_pixels * bi.n_samples;
-                CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                const auto raygen = raygen_kernel(sc);
-                raygen<<<(n + 255) / 256, 256, 0, st>>>(sc->d, rp, ps, bi, cam_sobol_p, X.queue[0].p, d_count, X.rays.p, d_nrays, sc->counters.p, sc->cam_mo,
-                                                        sc->env_res, lens_arg(sc, X));
-                launches++;
-                int rc = trace();
-                if (rc != PBRT_OK) return rc;
-                CK(cudaMemsetAsync(d_nrays, 0, 4, st));
-                cudaEvent_t e, f;
-                CK(scr->event(&e)); CK(scr->event(&f));
-                CK(cudaEventRecord(e, st));
-                const uint64_t total = (uint64_t)n * ao_n;
-                k_ao_shade<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(sc->d, rp, ps, bi, ao_n, p->ao_cos_sample ? 1u : 0u, sc->nib.p, n_chunks, sc->vdc.p,
-                                                                         sc->vdci.p, X.rays.p, X.ao_weight.p, d_nrays);
-                CK(cudaEventRecord(f, st));
-                sev.push_back(e); sev.push_back(f);
-                launches++;
-                if ((rc = trace()) != PBRT_OK) return rc;
-                k_ao_resolve<<<(n + 255) / 256, 256, 0, st>>>(ps, bi, ao_n, X.ao_weight.p, X.occl.p);
-                const auto resolve = resolve_kernel(sc);
-                resolve<<<(bi.n_pixels + 255) / 256, 256, 0, st>>>(rp, ps, bi, scr->filter_table.p, d_film, d_samples, X.cam_weight.p);
-                launches += 2;
-            }
-        CK(cudaGetLastError());
-        CK(cudaEventRecord(ev1, st));
-        CK(cudaStreamSynchronize(st));
-    } else if (share_pixels > 0) {
-        const uint64_t total_pixels = share_pixels;
-        // Camera samples in flight per batch.  2^24 (6 GB of wavefront state per stream context): every batch ends in one or two iterations
-        // that hold a few thousand rays and still last as long as one ray's chain of dependent fetches, so fewer, larger batches spend
-        // less of the frame in those tails (the statue and shares of its frame gain; Cornell and the conference scene are indifferent).
-        // Two contexts of 2^24 take 12 GB, well inside an 80 GB H100.
-        // Scenes with textured materials stay at 2^22: k_texture leaves a 496-byte lobe record per hit (8 GB per context at 2^24) that k_shade
-        // reads back through the class-sorted queue, and k_shade's time per slot grows with that working set.
-        static const int cap_log2_env = getenv("PB_BATCH_LOG2") ? std::min(26, std::max(10, atoi(getenv("PB_BATCH_LOG2")))) : 0;
-        const int cap_log2 = cap_log2_env ? cap_log2_env : (sc->d.n_textures ? 22 : 24);
-        const size_t CAP = (size_t)1 << cap_log2;
-        const uint32_t samples_per_batch = (uint32_t)std::min<size_t>(rp.spp, CAP);
-        const uint32_t pixels_per_batch = (uint32_t)std::min<uint64_t>(std::max<size_t>(1, CAP / samples_per_batch), total_pixels);
-        const size_t cap = (size_t)samples_per_batch * pixels_per_batch;
-        const uint64_t n_batches = ((rp.spp + samples_per_batch - 1) / samples_per_batch) * ((total_pixels + pixels_per_batch - 1) / pixels_per_batch);
-        // PB_SHADE_SPEC=0 turns the single-lobe instantiations of k_shade off (A/B switch; every class then runs the general one);
-        // =1 keeps only the Lambert one (round 2's first step)
-        static const int shade_spec = getenv("PB_SHADE_SPEC") ? atoi(getenv("PB_SHADE_SPEC")) : 2;
-        const bool plan_instanced = sc->d.n_instances > 0;
-        struct ShadeLaunch { int spec; uint32_t lo, hi; };
-        std::vector<ShadeLaunch> shade_plan;
-        if (sc->light_level >= 2) shade_plan.push_back({0, 1u, (uint32_t)PB_SHADE_CLASSES});
-        else {
-            uint32_t mask = sc->class_mask & ~1u, covered = 0;
-            const uint32_t first_general = PB_SPEC_PLASTIC + 1;
-            for (uint32_t c = 1; c < first_general && shade_spec; ++c) {
-                if (!(mask & (1u << c))) continue;
-                const bool have = c == 1 + LOBE_LAMBERT || (shade_spec >= 2 && !halton && !plan_instanced && (c == 1 + LOBE_SPEC_REFL || c == 1 + LOBE_FRESNEL_SPEC || c == 1 + LOBE_OREN_NAYAR ||
-                                                                                                    c == 1 + LOBE_MF_REFL || c == 1 + LOBE_FRESNEL_BLEND || c == PB_SPEC_PLASTIC));
-                if (!have) continue;
-                shade_plan.push_back({(int)c, c, c + 1});
-                covered |= 1u << c;
-            }
-            // the classes no specialised launch covers, as maximal runs, for the general instantiation
-            const uint32_t rest = mask & ~covered;
-            for (uint32_t c = 1; c < PB_SHADE_CLASSES;) {
-                if (!(rest & (1u << c))) { ++c; continue; }
-                uint32_t e = c;
-                while (e < PB_SHADE_CLASSES && (rest & (1u << e))) ++e;
-                shade_plan.push_back({0, c, e});
-                c = e;
-            }
-            // when no material has class 1, the null-material hits that k_sort files under class 1 (a shape without a material, or a
-            // moved instance under quirk Q7): folded into the Lambert launch when nothing lies between, else a launch of their own (the
-            // cheapest instantiation: no BSDF is touched).  An otherwise empty plan keeps that launch too: k_shade resets the counters
-            // the next iteration fills.
-            const uint32_t lam = 1 + LOBE_LAMBERT;
-            const bool null_hits = sc->has_null_material || (plan_instanced && p->instancing == PBRT_INSTANCING_REFERENCE);
-            if (!(mask & 2u) && (null_hits || shade_plan.empty())) {
-                bool folded = false;
-                if ((covered & (1u << lam)) && (mask & ((1u << lam) - 4u)) == 0u)
-                    for (ShadeLaunch& l : shade_plan) if (l.spec == (int)lam) { l.lo = 1; folded = true; }
-                if (!folded) shade_plan.insert(shade_plan.begin(), ShadeLaunch{shade_spec ? (int)lam : 0, 1u, 2u});
-            }
-        }
-        // Two batches in flight on two streams: k_trace and k_shade leave the SMs idle in different ways, so letting one batch
-        // trace while the other shades fills the SMs better than either alone.  Disabled for the roofline timing pass
-        // (PBRT_RENDER_SINGLE_STREAM: kernel durations must not be inflated by a co-resident kernel), when the queue
-        // has to be polled from the host (null materials), and when there is only one batch.
-        static const bool dual_env = !(getenv("PB_SINGLE_STREAM") && atoi(getenv("PB_SINGLE_STREAM")));
-        // ... and when an iteration is a single k_shade launch.  On an H100 at 400 W (DESIGN.md section 7) the statue, two launches per
-        // iteration, renders at 1 629-1 637 Mrays/s with two batches in flight against 1 574-1 585 with one; Cornell, one Lambert launch,
-        // cannot be told apart (2 873-2 953 against 2 902-2 969), so it keeps one stream.  PB_STREAMS = 1 keeps one batch in flight,
-        // PB_STREAMS >= 2 forces two.
-        // A textured frame is bound by k_texture's per-hit records (written once, read back by k_shade): a second batch in flight doubles that
-        // working set and loses.
-        const bool streams_forced = getenv("PB_STREAMS") && atoi(getenv("PB_STREAMS")) >= 2;
-        const bool dual = dual_env && !(p->flags & PBRT_RENDER_SINGLE_STREAM) && !null_paths && n_batches > 1 &&
-                          !(getenv("PB_STREAMS") && atoi(getenv("PB_STREAMS")) <= 1) && ((shade_plan.size() >= 2 && sc->d.n_textures == 0) || streams_forced);
-        static const int streams_env = getenv("PB_STREAMS") ? std::min(4, std::max(1, atoi(getenv("PB_STREAMS")))) : 2;
-        const int n_ctx = dual ? (int)std::min<uint64_t>((uint64_t)streams_env, n_batches) : 1;
+    if (R.share_pixels == 0) TRY(end_frame(R));
+    else if (direct) TRY(render_direct(sc, scr, R));
+    else if (p->integrator == PBRT_INTEGRATOR_AO) TRY(render_ao(sc, scr, R));
+    else TRY(render_path(sc, scr, R));
 
-        const int sm_count = sm_count_of(sc->device);
-        const bool count_work = (p->flags & PBRT_RENDER_COUNT_WORK) != 0;
-        const bool spatial = strategy == PBRT_LIGHTS_SPATIAL && nl > 0;
-
-        // ---- light grid geometry (SpatialLightDistribution::new lightdistrib.rs:127-150) / fixed distributions ----
-        int nv[3] = {1, 1, 1};
-        size_t nvox = 1;
-        if (spatial) {
-            float diag[3] = {sc->d.wb_max[0] - sc->d.wb_min[0], sc->d.wb_max[1] - sc->d.wb_min[1], sc->d.wb_max[2] - sc->d.wb_min[2]};
-            int me = (diag[0] > diag[1] && diag[0] > diag[2]) ? 0 : (diag[1] > diag[2] ? 1 : 2);
-            float bmax = diag[me];
-            for (int i = 0; i < 3; ++i) {
-                nv[i] = std::max(1, f2i_sat(roundf(diag[i] / bmax * 64.0f)));
-                nvox *= (size_t)nv[i];
-            }
-        }
-        // func + contrib + cdf + func_int of one voxel.  Dense tables for every voxel are the fast path (Cornell: 7 MB); with one
-        // light per emissive triangle they would be nvox x n_lights x 12 bytes (10 k emitters: 31 GB per stream context), so above
-        // the budget the tables become rows handed out on first touch (DLightGrid::row) and the render fails, rather than the
-        // allocation, should the paths visit more voxels than fit.
-        const size_t grid_row_bytes = (3 * std::max<size_t>(nl, 1) + 2) * sizeof(float);
-        const size_t grid_budget = lightgrid_budget();
-        const bool grid_sparse = spatial && nvox * grid_row_bytes > grid_budget;
-        const size_t grid_rows = grid_sparse ? std::max<size_t>(1, std::min(nvox, grid_budget / grid_row_bytes)) : nvox;
-        std::vector<float> fixed_f(nl, 1.0f), fixed_cdf;
-        float fixed_int = 0.0f;
-        if (!spatial && nl > 0) {
-            if (strategy == PBRT_LIGHTS_POWER)  // compute_light_power_distribution integrator.rs:574-584, diffuse.rs:85-93
-                for (uint32_t j = 0; j < nl; ++j) {
-                    const DLight& l = sc->h_lights[j];
-                    Sp pw;
-                    const Sp I = mksp(l.L[0], l.L[1], l.L[2]);
-                    if (l.kind == PBRT_LIGHT_POINT) pw = I * (4.0f * PB_PI);  // point.rs / spot.rs / distant.rs power()
-                    else if (l.kind == PBRT_LIGHT_SPOT) pw = I * 2.0f * PB_PI * (1.0f - 0.5f * (l.cos_falloff_start + l.cos_total_width));
-                    else if (l.kind == PBRT_LIGHT_DISTANT) pw = I * PB_PI * sc->d.world_radius * sc->d.world_radius;
-                    else if (l.kind == PBRT_LIGHT_INFINITE) pw = sc->h_env_power[j] * sp1(PB_PI * sc->d.world_radius * sc->d.world_radius);  // infinite.rs:349-355
-                    else if (l.kind == PBRT_LIGHT_GONIOMETRIC || l.kind == PBRT_LIGHT_PROJECTION) pw = sc->h_env_power[j];
-                    else pw = I * (l.two_sided ? 2.0f : 1.0f) * l.area * PB_PI;
-                    fixed_f[j] = lum(pw);
-                }
-            make_distribution(fixed_f, fixed_cdf, fixed_int);
-        }
-        CK(scr->filter_table.alloc(256));
-        CK(cudaMemcpyAsync(scr->filter_table.p, p->filter_table, 256 * 4, cudaMemcpyHostToDevice, st));
-
-        // Sobol' dimensions reachable by this render: 5 camera dims + 8 per shaded bounce; index bits: 2*log2(resolution)
-        // pixel bits + log2(spp) sample bits (sobol_interval_to_index)
-        uint32_t dims_needed = (uint32_t)std::min<uint64_t>(1024u, 5 + 8 * ((uint64_t)rp.max_depth + 1));
-        uint32_t log2_spp = 0;
-        while ((1u << log2_spp) < rp.spp) log2_spp++;
-        const uint32_t index_bits = std::min<uint32_t>(52u, 2u * rp.log2_res + log2_spp);
-        const uint32_t n_chunks = std::max<uint32_t>(1u, (index_bits + 3u) / 4u);
-        // this render's transposed nibble-table slice nibT[(chunk*16+e)*ds + dim], padded by 8 dimensions (pb_sobol.cuh)
-        const uint32_t sobol_ds = (dims_needed + 8u) | 1u;
-        {
-            std::vector<uint32_t>& T = scr->h_nibT;
-            T.assign((size_t)n_chunks * 16 * sobol_ds, 0u);
-            for (uint32_t c = 0; c < n_chunks; ++c)
-                for (uint32_t e = 0; e < 16; ++e)
-                    for (uint32_t d = 0; d < dims_needed; ++d) T[((size_t)c * 16 + e) * sobol_ds + d] = sc->h_nib[((size_t)d * PB_SOBOL_CHUNKS + c) * 16 + e];
-            CK(scr->nibT.alloc(T.size()));
-            CK(cudaMemcpyAsync(scr->nibT.p, T.data(), T.size() * 4, cudaMemcpyHostToDevice, st));
-        }
-        const bool stage_sobol = (size_t)sobol_ds * n_chunks * 64 <= PB_SMEM_SOBOL_BYTES;
-        const uint32_t sobol_cfg = sobol_ds | (stage_sobol ? 0x80000000u : 0u);
-        const size_t shade_smem = stage_sobol ? (size_t)sobol_ds * n_chunks * 64 : 0;
-        const uint32_t* shade_nib = scr->nibT.p;
-        const uint4* cam_sobol_p = nullptr;  // (on the caller's stream, ahead of ev_start: every context's k_raygen reads it)
-        CK(camera_sobol(scr, sc, rp, n_chunks, st, &cam_sobol_p));
-        launches += halton ? 0 : 1;
-        // persistent trace grid: the CTAs that are resident at once (half of them per stream when two batches overlap)
-        const bool instanced = sc->d.n_instances > 0;
-        const bool textured = sc->d.n_textures > 0;
-        TraceLauncher tl;
-        CK(tl.init(sc, count_work, sm_count));
-        // With batches in flight on several streams each stream's persistent trace grid takes 3/(2*n_ctx) of the resident CTAs -- 6 of 8
-        // per SM with two streams -- not an even 1/n_ctx share: a batch that traces while its partner shades or sorts cannot grow into the
-        // idle half, and an even share left it at half occupancy then.  When both trace at once, the CTAs that do not fit wait for free
-        // slots and take what is left of their queue.  On an H100 the statue rendered about 3 % faster than with 4 of 8 (DESIGN.md section 7).
-        tl.grid = sm_count * std::max(1, n_ctx > 1 ? std::max(tl.blocks_per_sm, 1) * 3 / (2 * n_ctx) : std::max(tl.blocks_per_sm, 1));
-        const int shade_grid = sm_count * (8 / n_ctx);
-        int shade_grid_spec = shade_grid;
-        if (shade_spec) {
-            int bps = 4;
-            cudaError_t oe;
-            constexpr int L = 1 + LOBE_LAMBERT;
-            if (halton) oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, true, true, L>, PB_SHADE_THREADS, 0)
-                            : sc->light_level == 0 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<0, true, false, L>, PB_SHADE_THREADS, 0)
-                                            : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, true, false, L>, PB_SHADE_THREADS, 0);
-            else oe = instanced ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, false, true, L>, PB_SHADE_THREADS, shade_smem)
-                     : sc->light_level == 0 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<0, false, false, L>, PB_SHADE_THREADS, shade_smem)
-                                     : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_shade<1, false, false, L>, PB_SHADE_THREADS, shade_smem);
-            CK(oe);
-            shade_grid_spec = sm_count * std::max(1, std::max(bps, 1) / n_ctx);
-        }
-        // the launches of one k_shade step: {specialisation, first class, one past the last class}.  Every single-lobe class the scene has
-        // gets its own instantiation (the Lambert one exists for every sampler / light / instancing combination, the others for the Sobol'
-        // sampler without instances: what the benchmark configurations run); class 0 ("nothing to shade") and the null-material hits of
-        // class 1 ride with the first launch; what is left goes to the general instantiation.
-        // ---- per-context buffers ---------------------------------------------------------------
-        struct Live {
-            DPaths ps; DLightGrid grid; TraceIO io;
-            uint32_t *counts, *d_err, *d_nrays, *d_cursor, *d_cls_count;
-            cudaStream_t s;
-            int cur;
-            int iter;
-        } live[4];
-        // PB_RAY_SORT=1 switches the coherence order of the ray queues on.  It shortens k_trace on Cornell and the conference scene
-        // (not on the 4.3 M-triangle statue), but the three bucketing kernels cost more than that (they re-read the 32 B ray records and fight over a few hot histogram bins), so it is OFF by default until
-        // the keys are produced by k_shade and the histogram is warp-aggregated (DESIGN.md section 9).
-        static const int ray_sort_mode = getenv("PB_RAY_SORT") ? atoi(getenv("PB_RAY_SORT")) : 0;  // 2: two-level scatter
-        static const bool ray_sort = ray_sort_mode != 0;
-        // PB_STATE_AOS=0: one dense array per state field instead of the three interleaved records (A/B switch)
-        static const bool state_aos = !(getenv("PB_STATE_AOS") && atoi(getenv("PB_STATE_AOS")) == 0);
-        // PB_RAY_PREP=1: k_rayprep computes the per-ray traversal constants ahead of k_trace (experiment, see pb_kernels.cuh)
-        static const bool ray_prep = getenv("PB_RAY_PREP") && atoi(getenv("PB_RAY_PREP"));
-        static const uint32_t ray_key_mask = getenv("PB_RAY_KEY_MASK") ? (uint32_t)strtoul(getenv("PB_RAY_KEY_MASK"), nullptr, 0) : 0x1fffu;
-        cudaEvent_t ev_start;
-        CK(scr->event(&ev_start));
-        CK(cudaEventRecord(ev_start, st));
-        for (int c = 0; c < n_ctx; ++c) {
-            BatchCtx& X = scr->ctx[c];
-            Live& V = live[c];
-            if (dual) {
-                if (!X.stream) CK(cudaStreamCreateWithFlags(&X.stream, cudaStreamNonBlocking));
-                V.s = X.stream;
-                CK(cudaStreamWaitEvent(V.s, ev_start, 0));
-            } else V.s = st;
-            if (state_aos) { for (int i = 0; i < 3; ++i) CK(X.rec[i].alloc(4 * cap)); CK(X.f4[3].alloc(cap)); }
-            else {
-                for (int i = 0; i < 9; ++i) CK(X.f4[i].alloc(cap));
-                CK(X.occl.alloc(cap)); CK(X.sobol.alloc(cap)); CK(X.dim.alloc(cap));
-            }
-            CK(X.rays.alloc(2 * 3 * cap));  // up to three rays (path, MIS, shadow) per slot and bounce
-            CK(X.pfilm.alloc(cap));
-            if (sc->cam_kind == PBRT_CAMERA_REALISTIC) CK(X.cam_weight.alloc(cap));
-            CK(X.queue[0].alloc(cap)); CK(X.queue[1].alloc(cap)); CK(X.counts.alloc(8 + 2 * PB_SHADE_CLASSES));
-            CK(X.cls_queue.alloc((size_t)PB_SHADE_CLASSES * cap));
-            CK(X.g_state.alloc(nvox)); CK(X.g_func.alloc(grid_rows * std::max<size_t>(nl, 1))); CK(X.g_cdf.alloc(grid_rows * (nl + 1)));
-            CK(X.g_fint.alloc(grid_rows)); CK(X.g_contrib.alloc(grid_rows * std::max<size_t>(nl, 1))); CK(X.g_request.alloc(nvox + 3));
-            if (grid_sparse) CK(X.g_row.alloc(nvox));
-            DPaths& ps = V.ps;
-            if (state_aos) {  // three 64-byte records per slot (pb_scene.cuh::DPaths)
-                auto f4 = [](float4* base, int k) { StridedView<float4> v; v.p = base + k; v.stride = 4; return v; };
-                float4 *A = X.rec[0].p, *B = X.rec[1].p, *C = X.rec[2].p;
-                // (L + flags stay a dense array: k_sort reads the flags word of every slot and k_resolve walks L in slot order)
-                ps.L = dense_view(X.f4[3].p); ps.ray_d = f4(A, 1); ps.beta = f4(A, 2);
-                ps.sobol.p = reinterpret_cast<uint2*>(A + 3); ps.sobol.stride = 8;
-                ps.dim.p = reinterpret_cast<uint32_t*>(A + 3) + 2; ps.dim.stride = 16;
-                ps.ld_light = f4(B, 0); ps.mis_d = f4(B, 1); ps.mis_f = f4(B, 2); ps.nee_beta = f4(B, 3);
-                ps.hit = f4(C, 0); ps.mis_hit = f4(C, 1);
-                ps.occl.p = reinterpret_cast<uint32_t*>(C + 2); ps.occl.stride = 16;
-                ps.path_rec = A;
-            } else {
-                ps.path_rec = nullptr;
-                ps.ray_d = dense_view(X.f4[0].p); ps.hit = dense_view(X.f4[1].p); ps.beta = dense_view(X.f4[2].p); ps.L = dense_view(X.f4[3].p);
-                ps.ld_light = dense_view(X.f4[4].p); ps.mis_hit = dense_view(X.f4[5].p); ps.mis_d = dense_view(X.f4[6].p); ps.mis_f = dense_view(X.f4[7].p);
-                ps.nee_beta = dense_view(X.f4[8].p);
-                ps.occl = dense_view(X.occl.p); ps.sobol = dense_view(X.sobol.p); ps.dim = dense_view(X.dim.p);
-            }
-            ps.p_film = X.pfilm.p;
-            if (instanced) { CK(X.hit_inst.alloc(cap)); CK(X.mis_inst.alloc(cap)); }
-            ps.hit_inst = X.hit_inst.p; ps.mis_inst = X.mis_inst.p;
-            ps.ray_diff = nullptr; ps.slot_mat = nullptr; ps.slot_frame = nullptr;
-            if (textured) {
-                CK(X.ray_diff.alloc(3 * cap)); CK(X.slot_mat.alloc(cap)); CK(X.slot_frame.alloc(2 * cap));
-                ps.ray_diff = X.ray_diff.p; ps.slot_mat = X.slot_mat.p; ps.slot_frame = X.slot_frame.p;
-            }
-            DLightGrid& g = V.grid;
-            std::memset(&g, 0, sizeof g);
-            g.n_lights = (int)nl;
-            g.nv[0] = nv[0]; g.nv[1] = nv[1]; g.nv[2] = nv[2];
-            g.state = X.g_state.p; g.func = X.g_func.p; g.cdf = X.g_cdf.p; g.func_int = X.g_fint.p;
-            g.contrib = X.g_contrib.p; g.request = X.g_request.p; g.n_request = X.g_request.p + nvox;
-            g.row = grid_sparse ? X.g_row.p : nullptr;
-            g.max_rows = (uint32_t)grid_rows;
-            CK(cudaMemsetAsync(g.state, 0, nvox * sizeof(int), V.s));
-            CK(cudaMemsetAsync(g.n_request, 0, 3 * sizeof(uint32_t), V.s));
-            if (grid_sparse) CK(cudaMemsetAsync(g.row, 0, nvox * sizeof(int), V.s));
-            if (!spatial && nl > 0) {
-                CK(cudaMemcpyAsync(g.func, fixed_f.data(), nl * 4, cudaMemcpyHostToDevice, V.s));
-                CK(cudaMemcpyAsync(g.cdf, fixed_cdf.data(), (nl + 1) * 4, cudaMemcpyHostToDevice, V.s));
-                CK(cudaMemcpyAsync(g.func_int, &fixed_int, 4, cudaMemcpyHostToDevice, V.s));
-            }
-            V.counts = X.counts.p; V.d_err = X.counts.p + 2; V.d_nrays = X.counts.p + 3; V.d_cursor = X.counts.p + 4; V.d_cls_count = X.counts.p + 8;
-            CK(cudaMemsetAsync(X.counts.p, 0, (8 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
-            std::memset(&V.io, 0, sizeof V.io);
-            V.io.rays = X.rays.p; V.io.hit = ps.hit; V.io.mis_hit = ps.mis_hit; V.io.occl = ps.occl;
-            V.io.hit_inst = ps.hit_inst; V.io.mis_inst = ps.mis_inst; V.io.instancing = rp.instancing;
-            V.cur = 0;
-            if (ray_sort) { CK(X.ray_keys.alloc(3 * cap)); CK(X.ray_perm.alloc(3 * cap)); CK(X.ray_hist.alloc(PB_RAY_KEYS)); }
-            if (ray_prep) CK(X.rays_pre.alloc(2 * 3 * cap));
-        }
-
-        // ---- one iteration (trace -> sort -> light grid -> shade) of the batch living in context c ----
-        // `stagger` (first iteration of a batch pair): context 1 starts tracing only when context 0 has finished its
-        // first trace, so that from then on one batch traces while the other shades
-        cudaEvent_t ev_stagger[4];
-        for (int i = 0; i < 4; ++i) CK(scr->event(&ev_stagger[i]));
-        auto enqueue_iteration = [&](int c, bool stagger) -> int {
-            BatchCtx& X = scr->ctx[c];
-            Live& V = live[c];
-            cudaStream_t s = V.s;
-            const int cur = V.cur;
-            uint32_t* c_in = V.counts + cur;
-            uint32_t* c_out = V.counts + (cur ^ 1);
-            uint32_t* cls_now = V.d_cls_count + PB_SHADE_CLASSES * (V.iter & 1);        // filled by this iteration's k_sort
-            uint32_t* cls_next = V.d_cls_count + PB_SHADE_CLASSES * ((V.iter + 1) & 1);  // cleared by this iteration's k_shade
-            if (stagger && c >= 1) CK(cudaStreamWaitEvent(s, ev_stagger[c - 1], 0));
-            // camera rays arrive in pixel order (coherent as they are); every later queue is bucketed by direction / origin
-            V.io.perm = nullptr;
-            if (ray_sort && V.iter > 0) {
-                CK(cudaMemsetAsync(X.ray_hist.p, 0, PB_RAY_KEYS * sizeof(uint32_t), s));
-                k_ray_hist<<<sm_count * 4, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p);
-                k_ray_scan<<<1, 1024, 0, s>>>(X.ray_hist.p);
-                if (ray_sort_mode == 2) k_ray_scatter2<<<sm_count * 8, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p, X.ray_perm.p);
-                else k_ray_scatter<<<sm_count * 8, 256, 0, s>>>(V.d_nrays, X.ray_keys.p, X.ray_hist.p, X.ray_perm.p);
-                launches += 3;
-                V.io.perm = X.ray_perm.p;
-            }
-            V.iter++;
-            cudaEvent_t a, b;
-            CK(scr->event(&a)); CK(scr->event(&b));
-            CK(cudaEventRecord(a, s));
-            V.io.pre = nullptr;
-            if (ray_prep) {  // (inside the k_trace event pair: its cost counts as traversal time)
-                k_rayprep<<<sm_count * 8, 256, 0, s>>>(X.rays.p, V.d_nrays, X.rays_pre.p);
-                launches++;
-                V.io.pre = X.rays_pre.p;
-            }
-            tl.launch(sc->d, V.io, V.d_nrays, V.d_cursor, sc->counters.p, s);
-            CK(cudaEventRecord(b, s));
-            if (stagger) CK(cudaEventRecord(ev_stagger[c], s));
-            tev.push_back(a); tev.push_back(b);
-            launches++; trace_launches++;
-            k_sort<<<sm_count * 8, 256, 0, s>>>(sc->d, V.ps, V.grid, spatial ? 1u : 0u, rp.instancing, X.queue[cur].p, c_in, X.cls_queue.p, (uint32_t)cap, cls_now, c_out,
-                                                V.d_nrays);
-            launches++;
-            if (textured) {  // V.iter == 1: the rays just traced are the camera rays, the only ones with differentials (none from an environment camera)
-                k_texture<<<sm_count * 8, 128, 0, s>>>(sc->d, rp, V.ps, X.queue[cur].p, c_in, V.iter == 1 && sc->cam_kind != PBRT_CAMERA_ENVIRONMENT ? 1u : 0u);
-                launches++;
-            }
-            if (spatial) {
-                if (sc->light_level >= 2) k_lightgrid_contrib<2><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
-                else k_lightgrid_contrib<1><<<sm_count * 2, 128, 0, s>>>(sc->d, V.grid, sc->halton.p);
-                k_lightgrid_build<<<sm_count, 128, 0, s>>>(V.grid);
-                launches += 2;
-            }
-            cudaEvent_t e, f;
-            CK(scr->event(&e)); CK(scr->event(&f));
-            CK(cudaEventRecord(e, s));
-#define PB_SHADE_ARGS(lo, hi) (sc->d, rp, V.ps, V.grid, shade_nib, sobol_cfg, n_chunks, X.cls_queue.p, (uint32_t)cap, cls_now, X.queue[cur ^ 1].p, c_out, \
-                              X.rays.p, V.d_nrays, sc->counters.p, V.d_err, ray_sort ? X.ray_keys.p : nullptr, ray_key_mask, V.d_cursor,    \
-                              spatial ? V.grid.n_request : nullptr, cls_next, (uint32_t)(lo), (uint32_t)(hi))
-#define PB_SHADE_LAUNCH(SPEC, grid, lo, hi)                                                                                                   \
-    do {                                                                                                                                      \
-        /* instanced scenes take the general-light variants (an instanced scene lit by area lights alone is rare enough) */                   \
-        if (halton) {                                                                                                                         \
-            if (instanced) k_shade<1, true, true, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                            \
-            else if (sc->light_level == 0) k_shade<0, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                   \
-            else k_shade<1, true, false, SPEC><<<grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(lo, hi);                                     \
-        } else {                                                                                                                              \
-            if (instanced) k_shade<1, false, true, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                  \
-            else if (sc->light_level == 0) k_shade<0, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);         \
-            else k_shade<1, false, false, SPEC><<<grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(lo, hi);                           \
-        }                                                                                                                                     \
-        launches++;                                                                                                                           \
-    } while (0)
-            for (const ShadeLaunch& sl : shade_plan) {
-                if (sc->light_level >= 2) {  // image lights: only the general instantiation has them (one launch over every class)
-                    if (halton && instanced) k_shade<2, true, true, 0><<<shade_grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
-                    else if (halton) k_shade<2, true, false, 0><<<shade_grid, PB_SHADE_THREADS, 0, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
-                    else if (instanced) k_shade<2, false, true, 0><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
-                    else k_shade<2, false, false, 0><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);
-                    launches++;
-                    continue;
-                }
-                switch (sl.spec) {
-                    case 1 + LOBE_LAMBERT: PB_SHADE_LAUNCH(1 + LOBE_LAMBERT, shade_grid_spec, sl.lo, sl.hi); break;
-#define PB_SHADE_SOBOL_ONLY(SPEC)                                                                                                                         \
-    do {                                                                                                                                                  \
-        if (sc->light_level == 0) k_shade<0, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                   \
-        else k_shade<1, false, false, SPEC><<<shade_grid, PB_SHADE_THREADS, shade_smem, s>>>PB_SHADE_ARGS(sl.lo, sl.hi);                                \
-        launches++;                                                                                                                                       \
-    } while (0)
-                    case 1 + LOBE_SPEC_REFL: PB_SHADE_SOBOL_ONLY(1 + LOBE_SPEC_REFL); break;
-                    case 1 + LOBE_FRESNEL_SPEC: PB_SHADE_SOBOL_ONLY(1 + LOBE_FRESNEL_SPEC); break;
-                    case 1 + LOBE_OREN_NAYAR: PB_SHADE_SOBOL_ONLY(1 + LOBE_OREN_NAYAR); break;
-                    case 1 + LOBE_MF_REFL: PB_SHADE_SOBOL_ONLY(1 + LOBE_MF_REFL); break;
-                    case 1 + LOBE_FRESNEL_BLEND: PB_SHADE_SOBOL_ONLY(1 + LOBE_FRESNEL_BLEND); break;
-                    case PB_SPEC_PLASTIC: PB_SHADE_SOBOL_ONLY(PB_SPEC_PLASTIC); break;
-#undef PB_SHADE_SOBOL_ONLY
-                    default: PB_SHADE_LAUNCH(0, shade_grid, sl.lo, sl.hi); break;
-                }
-            }
-#undef PB_SHADE_LAUNCH
-#undef PB_SHADE_ARGS
-            CK(cudaEventRecord(f, s));
-            sev.push_back(e); sev.push_back(f);
-            V.cur ^= 1;
-            return PBRT_OK;
-        };
-        auto enqueue_begin = [&](int c, const BatchInfo& bi) -> int {
-            BatchCtx& X = scr->ctx[c];
-            Live& V = live[c];
-            V.cur = 0;
-            V.iter = 0;
-            uint32_t n = bi.n_pixels * bi.n_samples;
-            // ray count, ray cursor, both sets of class counts (and the voxel requests): from here on the kernels reset them for each other
-            CK(cudaMemsetAsync(V.d_nrays, 0, (5 + 2 * PB_SHADE_CLASSES) * sizeof(uint32_t), V.s));
-            if (spatial) CK(cudaMemsetAsync(V.grid.n_request, 0, 4, V.s));
-            const auto raygen = raygen_kernel(sc);
-            raygen<<<(n + 255) / 256, 256, 0, V.s>>>(sc->d, rp, V.ps, bi, cam_sobol_p, X.queue[0].p, V.counts, X.rays.p, V.d_nrays, sc->counters.p, sc->cam_mo,
-                                                      sc->env_res, lens_arg(sc, X));
-            launches++;
-            return PBRT_OK;
-        };
-        auto enqueue_end = [&](int c, const BatchInfo& bi) -> int {
-            Live& V = live[c];
-            const auto resolve = resolve_kernel(sc);
-            resolve<<<(bi.n_pixels + 255) / 256, 256, 0, V.s>>>(rp, V.ps, bi, scr->filter_table.p, d_film, d_samples, scr->ctx[c].cam_weight.p);
-            launches++;
-            return PBRT_OK;
-        };
-
-        // ---- batches ------------------------------------------------------------------------------
-        std::vector<BatchInfo> batches;
-        for (uint32_t s0 = 0; s0 < rp.spp; s0 += samples_per_batch)
-            for (uint64_t pix0 = 0; pix0 < total_pixels; pix0 += pixels_per_batch) {
-                BatchInfo bi;
-                bi.first_pixel = (uint32_t)pix0;
-                bi.n_pixels = (uint32_t)std::min<uint64_t>(pixels_per_batch, total_pixels - pix0);
-                bi.first_sample = s0;
-                bi.n_samples = std::min(samples_per_batch, rp.spp - s0);
-                bi.n_samples_magic = magic_of(bi.n_samples);
-                batches.push_back(bi);
-            }
-        const uint32_t iters = rp.max_depth + 1;
-        int rc = PBRT_OK;
-        since("setup done");
-        if (null_paths) {
-            // paths can pass through null surfaces without counting a bounce, so the number of iterations is only known on the
-            // device.  The queue length is read one iteration late (see the DirectLighting loop): the iteration queued past the end
-            // runs over empty queues, like the tail iterations of the fixed-length loop below.
-            uint32_t* h_poll = nullptr;
-            cudaEvent_t poll_ev[2];
-            CK(scr->poll_words(&h_poll));
-            CK(scr->event(&poll_ev[0])); CK(scr->event(&poll_ev[1]));
-            const uint32_t lag = poll_lag();
-            for (const BatchInfo& bi : batches) {
-                if ((rc = enqueue_begin(0, bi)) != PBRT_OK) return rc;
-                for (uint32_t it = 0;; ++it) {
-                    if ((rc = enqueue_iteration(0, false)) != PBRT_OK) return rc;
-                    CK(cudaMemcpyAsync(&h_poll[4u + (it & 1u)], live[0].counts + live[0].cur, 4, cudaMemcpyDeviceToHost, live[0].s));
-                    CK(cudaEventRecord(poll_ev[it & 1u], live[0].s));
-                    if (it >= lag) {
-                        CK(cudaEventSynchronize(poll_ev[(it - lag) & 1u]));
-                        if (h_poll[4u + ((it - lag) & 1u)] == 0u) break;
-                    }
-                }
-                if ((rc = enqueue_end(0, bi)) != PBRT_OK) return rc;
-            }
-        } else {
-            // batches are dealt to the contexts round robin; the host interleaves the two streams' launches at
-            // iteration granularity so both always have work queued
-            for (size_t b0 = 0; b0 < batches.size(); b0 += (size_t)n_ctx) {
-                const int nb = (int)std::min<size_t>((size_t)n_ctx, batches.size() - b0);
-                for (int c = 0; c < nb; ++c) if ((rc = enqueue_begin(c, batches[b0 + c])) != PBRT_OK) return rc;
-                for (uint32_t it = 0; it < iters; ++it)
-                    for (int c = 0; c < nb; ++c) if ((rc = enqueue_iteration(c, dual && nb >= 2 && it == 0)) != PBRT_OK) return rc;
-                for (int c = 0; c < nb; ++c) if ((rc = enqueue_end(c, batches[b0 + c])) != PBRT_OK) return rc;
-            }
-        }
-        CK(cudaGetLastError());
-        since("all batches enqueued");
-        // join the side streams back into the caller's stream
-        if (dual)
-            for (int c = 0; c < n_ctx; ++c) {
-                cudaEvent_t done;
-                CK(scr->event(&done));
-                CK(cudaEventRecord(done, live[c].s));
-                CK(cudaStreamWaitEvent(st, done, 0));
-            }
-        uint32_t err = 0, err1 = 0, errs[4] = {0, 0, 0, 0}, grid_full[4] = {0, 0, 0, 0};
-        for (int c = 0; c < n_ctx; ++c) CK(cudaMemcpyAsync(&errs[c], live[c].d_err, 4, cudaMemcpyDeviceToHost, st));
-        if (grid_sparse)
-            for (int c = 0; c < n_ctx; ++c) CK(cudaMemcpyAsync(&grid_full[c], live[c].grid.n_request + 2, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaEventRecord(ev1, st));
-        CK(cudaStreamSynchronize(st));
-        since("final sync");
-        if (grid_full[0] | grid_full[1] | grid_full[2] | grid_full[3])
-            return fail(PBRT_E_UNSUPPORTED, "spatial light distribution: the paths touch more voxels than the table budget holds (PB_LIGHTGRID_BYTES, "
-                                            "default 4 GiB per stream context); render with the power or uniform light strategy");
-        err = errs[0] | errs[1] | errs[2] | errs[3];
-        if (err | err1) return fail(PBRT_E_UNSUPPORTED, halton ? "HaltonSampler can only sample 1000 dimensions (halton.rs:256-262)"
-                                                               : "SobolSampler can only sample up to 1024 dimensions (sobol.rs:119-124)");
-    } else {
-        CK(cudaEventRecord(ev1, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    g_launches += launches;
+    g_launches += R.launches;
     if (stats) {
         std::memset(stats, 0, sizeof *stats);
         DCounters c;
@@ -2671,12 +2680,12 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
         stats->nodes_visited = c.nodes_visited; stats->tris_tested = c.tris_tested; stats->light_tri_tests = c.light_tri_tests;
         stats->shade_slots = c.shade_slots; stats->shaded_vertices = c.shaded_vertices;
         float ms = 0.0f;
-        CK(cudaEventElapsedTime(&ms, ev0, ev1));
+        CK(cudaEventElapsedTime(&ms, ev0, R.ev1));
         stats->ms_total = ms;
-        for (size_t i = 0; i + 1 < tev.size(); i += 2) { float m = 0; cudaEventElapsedTime(&m, tev[i], tev[i + 1]); stats->ms_trace += m; }
-        for (size_t i = 0; i + 1 < sev.size(); i += 2) { float m = 0; cudaEventElapsedTime(&m, sev[i], sev[i + 1]); stats->ms_shade += m; }
-        stats->trace_launches = trace_launches;
-        stats->kernel_launches = launches;
+        for (size_t i = 0; i + 1 < R.tev.size(); i += 2) { float m = 0; cudaEventElapsedTime(&m, R.tev[i], R.tev[i + 1]); stats->ms_trace += m; }
+        for (size_t i = 0; i + 1 < R.sev.size(); i += 2) { float m = 0; cudaEventElapsedTime(&m, R.sev[i], R.sev[i + 1]); stats->ms_shade += m; }
+        stats->trace_launches = R.trace_launches;
+        stats->kernel_launches = R.launches;
     }
 #ifdef PB_TRACE_PHASE_CLOCKS
     {
@@ -2688,7 +2697,7 @@ static int render_impl(PbrtScene* sc, const PbrtRenderParams* p, const Share& sh
                 ph[0], ph[1], ph[2], ph[3], ph[4]);
     }
 #endif
-    since("stats + event teardown");
+    R.since("stats + event teardown");
     return PBRT_OK;
 }
 
@@ -2852,8 +2861,9 @@ int pbrt_gpu_render_samples(PbrtScene* scene, const PbrtRenderParams* params, co
     return PBRT_OK;
 }
 
+// The ray-cast entry points' input rays on the device, and the TraceIO that names them
 static int rays_common(PbrtScene* sc, uint32_t n, const float* o, const float* d, const float* t_max, DevBuf<float>& bo, DevBuf<float>& bd,
-                       DevBuf<float>& bt) {
+                       DevBuf<float>& bt, TraceIO& io) {
     CK(cudaSetDevice(sc->device));
     CK(bo.alloc(3 * (size_t)n + 1)); CK(bd.alloc(3 * (size_t)n + 1)); CK(bt.alloc((size_t)n + 1));
     CK(cudaMemcpy(bo.p, o, 3 * (size_t)n * 4, cudaMemcpyHostToDevice));
@@ -2861,11 +2871,34 @@ static int rays_common(PbrtScene* sc, uint32_t n, const float* o, const float* d
     CK(cudaMemcpy(bt.p, t_max, (size_t)n * 4, cudaMemcpyHostToDevice));
     CK(sc->counters.alloc(1));
     CK(cudaMemset(sc->counters.p, 0, sizeof(DCounters)));
-    if (sc->d.mesh_alpha) {  // the alpha test walks a texture graph: stack frames above the default limit (see render_impl)
-        size_t cur = 0;
-        CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
-        if (cur < 4096) CK(cudaDeviceSetLimit(cudaLimitStackSize, 4096));
-    }
+    if (sc->d.mesh_alpha) TRY(raise_stack_limit());  // the alpha test walks a texture graph
+    std::memset(&io, 0, sizeof io);
+    io.o = bo.p; io.d = bd.p; io.tmax = bt.p;
+    return PBRT_OK;
+}
+// k_trace MODE 1 (closest hit) or 2 (any hit) over the n rays of `io` on the legacy stream, inside an event pair (*ms).  Instanced
+// scenes: PBRT_INSTANCING_REFERENCE semantics (the ray-cast entry points carry no render parameters).
+static int cast_rays(PbrtScene* sc, int mode, uint32_t n, const TraceIO& io, float* ms) {
+    const DScene& d = sc->d;
+    TraceKernel k;
+    if (mode == 1) k = d.mesh_alpha ? (d.n_instances ? k_trace<true, 1, false, true, true> : k_trace<true, 1, false, false, true>)
+                                    : (d.n_instances ? k_trace<true, 1, false, true> : k_trace<true, 1, false>);
+    else k = d.mesh_alpha ? (d.n_instances ? k_trace<true, 2, false, true, true> : k_trace<true, 2, false, false, true>)
+                          : (d.n_instances ? k_trace<true, 2, false, true> : k_trace<true, 2, false>);
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    int grid = (int)std::min<uint64_t>(((uint64_t)n + PB_TRACE_THREADS - 1) / PB_TRACE_THREADS, (uint64_t)sm_count_of(sc->device) * 16);
+    CK(cudaEventRecord(e0));
+    DevBuf<uint32_t> cursor;
+    CK(cursor.alloc(1));
+    CK(cudaMemset(cursor.p, 0, 4));
+    k<<<grid, PB_TRACE_THREADS>>>(d, io, nullptr, n, cursor.p, sc->counters.p);
+    CK(cudaEventRecord(e1));
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    g_launches++;
+    cudaEventElapsedTime(ms, e0, e1);
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
     return PBRT_OK;
 }
 static int rays_stats(PbrtScene* sc, PbrtStats* stats, float ms) {
@@ -2886,32 +2919,12 @@ int pbrt_gpu_intersect(PbrtScene* sc, uint32_t n, const float* o, const float* d
     if (n == 0) { if (stats) std::memset(stats, 0, sizeof *stats); return PBRT_OK; }
     DevBuf<float> bo, bd, bt, dt, db;
     DevBuf<int> dp;
-    int rc = rays_common(sc, n, o, d, t_max, bo, bd, bt);
-    if (rc != PBRT_OK) return rc;
-    CK(dp.alloc(n)); CK(dt.alloc(n)); CK(db.alloc(3 * (size_t)n));
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    int grid = (int)std::min<uint64_t>(((uint64_t)n + PB_TRACE_THREADS - 1) / PB_TRACE_THREADS, (uint64_t)sm_count_of(sc->device) * 16);
-    CK(cudaEventRecord(e0));
-    DevBuf<uint32_t> cursor;
-    CK(cursor.alloc(1));
-    CK(cudaMemset(cursor.p, 0, 4));
     TraceIO io;
-    std::memset(&io, 0, sizeof io);
-    io.o = bo.p; io.d = bd.p; io.tmax = bt.p; io.out_prim = dp.p; io.out_t = dt.p; io.out_b = db.p;
-    // instanced scenes: PBRT_INSTANCING_REFERENCE semantics (the ray-cast entry points carry no render parameters)
-    if (sc->d.mesh_alpha) {
-        if (sc->d.n_instances) k_trace<true, 1, false, true, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-        else k_trace<true, 1, false, false, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    } else if (sc->d.n_instances) k_trace<true, 1, false, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    else k_trace<true, 1, false><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    CK(cudaEventRecord(e1));
-    CK(cudaGetLastError());
-    CK(cudaDeviceSynchronize());
-    g_launches++;
+    TRY(rays_common(sc, n, o, d, t_max, bo, bd, bt, io));
+    CK(dp.alloc(n)); CK(dt.alloc(n)); CK(db.alloc(3 * (size_t)n));
+    io.out_prim = dp.p; io.out_t = dt.p; io.out_b = db.p;
     float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    TRY(cast_rays(sc, 1, n, io, &ms));
     CK(cudaMemcpy(prim, dp.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(t, dt.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(b, db.p, 3 * (size_t)n * 4, cudaMemcpyDeviceToHost));
@@ -2923,31 +2936,12 @@ int pbrt_gpu_intersect_p(PbrtScene* sc, uint32_t n, const float* o, const float*
     if (n == 0) { if (stats) std::memset(stats, 0, sizeof *stats); return PBRT_OK; }
     DevBuf<float> bo, bd, bt;
     DevBuf<unsigned char> docc;
-    int rc = rays_common(sc, n, o, d, t_max, bo, bd, bt);
-    if (rc != PBRT_OK) return rc;
-    CK(docc.alloc(n));
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    int grid = (int)std::min<uint64_t>(((uint64_t)n + PB_TRACE_THREADS - 1) / PB_TRACE_THREADS, (uint64_t)sm_count_of(sc->device) * 16);
-    CK(cudaEventRecord(e0));
-    DevBuf<uint32_t> cursor;
-    CK(cursor.alloc(1));
-    CK(cudaMemset(cursor.p, 0, 4));
     TraceIO io;
-    std::memset(&io, 0, sizeof io);
-    io.o = bo.p; io.d = bd.p; io.tmax = bt.p; io.out_occ = docc.p;
-    if (sc->d.mesh_alpha) {
-        if (sc->d.n_instances) k_trace<true, 2, false, true, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-        else k_trace<true, 2, false, false, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    } else if (sc->d.n_instances) k_trace<true, 2, false, true><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    else k_trace<true, 2, false><<<grid, PB_TRACE_THREADS>>>(sc->d, io, nullptr, n, cursor.p, sc->counters.p);
-    CK(cudaEventRecord(e1));
-    CK(cudaGetLastError());
-    CK(cudaDeviceSynchronize());
-    g_launches++;
+    TRY(rays_common(sc, n, o, d, t_max, bo, bd, bt, io));
+    CK(docc.alloc(n));
+    io.out_occ = docc.p;
     float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    TRY(cast_rays(sc, 2, n, io, &ms));
     CK(cudaMemcpy(occluded, docc.p, n, cudaMemcpyDeviceToHost));
     return rays_stats(sc, stats, ms);
 }
